@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — latent-frames/sec through the full GCD denoising hot path on B200.
+"""bench.py — latent-frames/sec through the full GCD denoising hot path on H100.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload kubric|pardom|direct50]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload kubric|pardom|direct50] [--dump-outputs DIR]
 
 A "step" = one pass of the hot path over one batch: per GPU ONE clip of 14 latent frames, 72x128 (576x1024 px):
 25 EDM/Euler steps of the CFG-doubled SVD VideoUNet (28 frames per forward) + the temporal VAE decode of the 14 frames
@@ -13,8 +13,10 @@ JSON line (rank 0): `value` = whole-job latent-frames/s with inputs resident in 
 `e2e` = same metric through the public API gcd_b200.pipeline.GCDHotPath.sample_video with pinned HOST inputs and a
 device->host read of the decoded frames inside the timed region; `roofline` = tensor-core roofline of the dominant kernel
 class (tc_gemm implicit-GEMM conv/linear) from CUDA events on the launching stream + whole-path fraction; `cpu_baseline` =
-the CPU oracle port (oracle/gcd_oracle.py) timed on this box's host cores on a bounded sample.
-`--impl reference` times only that CPU port (the reference's own PyTorch code cannot travel to the GPU box).
+the CPU oracle port (oracle/gcd_oracle.py) timed on this host's cores on a bounded sample.
+`--impl reference` times only that CPU port (the reference's own PyTorch code is not part of this repository).
+`--dump-outputs DIR` writes what the last timed step computed (the sampled latents and a stride-2 subsample of the decoded
+frames, float32 .npy) so that two builds can be compared output for output: the inputs are seeded, identical from run to run.
 """
 import argparse
 import json
@@ -45,11 +47,11 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(tflops=d["bf16_tflops_sustained"], burst=d["bf16_tflops"], hbm=d["hbm_gbs"], src="measured (MEASURED_PEAKS.json, sustained bf16)")
-    return dict(tflops=1400.0, burst=1590.0, hbm=6650.0, src="fallback (B200_PROFILING.md)")
+    return dict(tflops=989.0, burst=989.0, hbm=3350.0, src="NVIDIA H100 SXM data sheet (dense fp16, 700 W card), not measured")
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle-reason samples during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle-reason samples during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -93,8 +95,7 @@ def _cpu_leg_worker(spec_json):
     from oracle import gcd_oracle as O
     a = json.loads(spec_json)
     unet_cfg, vae_cfg, (h, w), (vh, vw) = a["unet_cfg"], a["vae_cfg"], a["lat_hw"], a["vae_hw"]
-    # Measured on the pool's 128-vCPU B200 hosts (tools/cpu_threads.py, same UNet sample): 16 threads 1.9 s, 32 threads
-    # 2.1 s, 64 threads 3.9 s, 128 threads 121 s (the cgroup quota is far below 128 cores) -> use the fastest setting.
+    # at most 32 threads: on hosts whose CPU quota is below their core count more threads run slower (tools/cpu_threads.py)
     cores = min(os.cpu_count() or 1, 32)
     torch.set_num_threads(cores)
     unet_state = synthetic.seeded_state(spec.unet_param_shapes(unet_cfg), seed=0)
@@ -146,17 +147,21 @@ def cpu_oracle_sample(unet_cfg, vae_cfg, steps, lat_hw=(LAT_H, LAT_W)):
     small warm-up call (thread pool / allocator). One clip = `steps` such forwards + one decode; every sampler step runs the
     identical network on identically shaped inputs, so clip time = steps x t_forward + t_decode ("extrapolated from 1 step":
     a full 25-step clip is ~1 h of host time). The same routine serves `cpu_baseline` and `--impl reference`, so the two legs
-    agree by construction. The measurement runs in a child process with a time limit (GCD_CPU_LEG_TIMEOUT, default 900 s; the full-size sample takes ~5 min on the pool's hosts);
-    if the full-size sample cannot run on this host (memory limit, time), a bounded sample (latent 16x24 / decode 8x8) is timed
-    instead and scaled by the exact algorithmic-FLOP ratios — and labelled as such.
+    agree by construction. The full-size sample takes minutes of host time, so it runs only when GCD_CPU_LEG_TIMEOUT (seconds)
+    is set, in a child process with that time limit. Otherwise, or if the full-size sample cannot run on this host (memory
+    limit, time), a bounded sample (latent 16x24 / decode 8x8) is timed instead and scaled by the exact algorithmic-FLOP
+    ratios — and labelled as such.
     Returns (latent_frames_per_s, description, cores, seconds_measured)."""
     from gcd_b200 import flops
     key = (tuple(sorted((k, str(v)) for k, v in unet_cfg.items())), tuple(sorted((k, str(v)) for k, v in vae_cfg.items())), steps, lat_hw)
     if key in _CPU_CACHE:
         return _CPU_CACHE[key]
     h, w = lat_hw
-    tmo = int(os.environ.get("GCD_CPU_LEG_TIMEOUT", "900"))
-    res, err = _run_cpu_leg(unet_cfg, vae_cfg, (h, w), (h, w), tmo)
+    tmo = os.environ.get("GCD_CPU_LEG_TIMEOUT")
+    if tmo:
+        res, err = _run_cpu_leg(unet_cfg, vae_cfg, (h, w), (h, w), int(tmo))
+    else:
+        res, err = None, "not requested: set GCD_CPU_LEG_TIMEOUT to time it"
     if res is not None:
         tu, tv, cores = res["tu"], res["tv"], res["cores"]
         desc = (f"1 CFG UNet forward (28 frames, latent {h}x{w}: {tu:.1f} s) + 1 VAE decode of 14 frames at latent {h}x{w} "
@@ -201,7 +206,7 @@ def run_reference(args, wl):
             "config": {"workload": wl["name"], "latent": [T_FRAMES, 4, lat[0], lat[1]], "sampler_steps": wl["steps"],
                        "measured_once": True,
                        "impl_note": "CPU port of the reference PyTorch path (oracle/gcd_oracle.py) at the workload's own shapes; "
-                                    "the reference itself is pure Python under /root/reference and cannot travel to the GPU box"},
+                                    "the reference itself is not part of this repository"},
             "cpu_baseline": {"value": v, "unit": "latent-frames/s", "cores": cores, "kind": "port", "sample": desc},
             "e2e": {"value": v, "unit": "latent-frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line), flush=True)
@@ -210,7 +215,7 @@ def run_reference(args, wl):
 # ------------------------------------------------------------------------------------------------------ extra workloads
 def run_extra_workloads(args, wl, pipe, ust, dev, rank, world, lat, timed, gathered):
     """BASELINE.json configs 3 and 4 and the single-clip latency mode, measured in the same process right after the main
-    line so the driver's N = 1/2/4/8 runs record them (one clip per rank each, CUDA events, max over ranks):
+    line so that runs on N = 1/2/4/8 GPUs record them (one clip per rank each, CUDA events, max over ranks):
       direct50     config 4: Kubric-4D direct max180 — 50 Euler steps, guider max scale 2.5 (pretrained/*.yaml:135), + decode,
                    clips sharded one per rank + the NCCL gather of the latents;
       pardom       config 3: ParallelDomain-4D network (no auxiliary embedding), 25 steps + decode, same sharding;
@@ -273,7 +278,11 @@ def run_extra_workloads(args, wl, pipe, ust, dev, rank, world, lat, timed, gathe
                                    "config": "one clip, CFG pair split over ranks 0/1, one NCCL all_gather of the network "
                                              "output per step; 25 steps + decode on rank 0"}
         dist.barrier()
-    # ---- config 3: ParDom network = the Kubric state without the auxiliary-embedding tensors (seeded per tensor name)
+    # ---- config 3: ParDom network = the Kubric state without the auxiliary-embedding tensors (seeded per tensor name).
+    # Two full-width networks with their workspaces and the decoder's do not fit in 80 GB: the Kubric one leaves the device.
+    del p50
+    pipe.unet.invalidate()
+    pipe.unet.to("cpu")
     pcfg = spec.UNET_PARDOM
     shapes = spec.unet_param_shapes(pcfg)
     pst = {k: ust[k] for k in shapes} if ust is not None else synthetic.seeded_state(shapes, seed=0)
@@ -286,6 +295,30 @@ def run_extra_workloads(args, wl, pipe, ust, dev, rank, world, lat, timed, gathe
 
 
 # ------------------------------------------------------------------------------------------------------ product arm
+def dump_outputs(out_dir, last):
+    """The arrays a caller of the timed path receives from its last step, as float32 .npy: the sampled latents [14, 4, H, W]
+    in full and the decoded frames [14, 3, 8H, 8W] at every 2nd pixel row and column (the full frames are 99 MB)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"latents": last["latents"]}
+    if last.get("frames") is not None:
+        arrays["frames_stride2"] = last["frames"][:, :, ::2, ::2]
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
+
+
+def gpu_info(index):
+    """Name and power limit of the card: part of every number this script reports."""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                           capture_output=True, text=True, timeout=30)
+        info["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.TimeoutExpired):
+        pass
+    return info
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -297,6 +330,8 @@ def main():
     ap.add_argument("--no-decode", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--cpu-leg", default=None, help=argparse.SUPPRESS)
     ap.add_argument("--no-extra", action="store_true", help="skip the extra_workloads block (BASELINE configs 3/4, CFG-parallel)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     ap.add_argument("--profile-run", action="store_true",
                     help="for ncu: exactly --warmup/--steps resident steps, no e2e / instrumented / CPU passes, no JSON claims")
     args = ap.parse_args()
@@ -338,11 +373,14 @@ def main():
     d2h = frames_host.numel() * 4
     gathered = [torch.empty(T_FRAMES, 4, LH, LW, device=dev) for _ in range(world)] if world > 1 else None
 
+    last = {}
+
     def step_resident(collective=True):
         z = pipe.sample_latents(dx.clone(), dc, duc)
         fr = None if args.no_decode else pipe.decode_first_stage(z)
         if world > 1 and collective:
             dist.all_gather(gathered, z.contiguous())     # the path's only collective: final gather over NVLink
+        last["latents"], last["frames"] = z, fr
         return z, fr
 
     def step_e2e():
@@ -379,24 +417,20 @@ def main():
         if rank == 0:
             print(json.dumps({"profile_run": True, "ms_per_step_under_profiler": ms / args.steps}))
         return
-    for _ in range(max(args.warmup, 3)):
+    for _ in range(max(args.warmup, 1)):       # the first clip allocates the workspaces and captures the UNet's CUDA graph
         step_resident()
     clocks = ClockSampler(local) if rank == 0 else None
     l0 = ops.launch_count()
     ms = timed(step_resident, args.steps)
     launches = ops.launch_count() - l0
     clk = clocks.stop() if clocks else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     step_e2e()
     ms_e2e = timed(step_e2e, args.steps)
 
-    extra = None if args.no_extra else run_extra_workloads(args, wl, pipe, ust, dev, rank, world, (LH, LW), timed, gathered)
-
-    frames_total = world * args.steps * T_FRAMES
-    value = frames_total / (ms / 1e3)
-    e2e_value = frames_total / (ms_e2e / 1e3)
-
-    # ---- per-kernel-class roofline (one extra, untimed, instrumented step on rank 0)
-    line = None
+    # ---- per-kernel-class roofline: one extra, untimed, instrumented step on rank 0 (before the extra workloads, which
+    # release this network's device memory)
     if rank == 0:
         pk = measured_peaks()
         g0, g1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -406,17 +440,22 @@ def main():
             g1.record()
         summ = prof.summary()
         prof_wall_ms = g0.elapsed_time(g1)        # eager, per-launch events: slower than the timed (graph-replay) steps
+
+    extra = None if args.no_extra else run_extra_workloads(args, wl, pipe, ust, dev, rank, world, (LH, LW), timed, gathered)
+
+    frames_total = world * args.steps * T_FRAMES
+    value = frames_total / (ms / 1e3)
+    e2e_value = frames_total / (ms_e2e / 1e3)
+
+    line = None
+    if rank == 0:
         tc = summ.get("tc_gemm", dict(ms=1e-9, flops=0.0, launches=0))
         tot_ms = sum(d["ms"] for d in summ.values())
         tc_tflops = tc["flops"] / (tc["ms"] / 1e3) / 1e12
         per_frame = flops.clip_flops(unet_cfg, vae_cfg, T_FRAMES, LH, LW, wl["steps"]) / T_FRAMES
         path_tflops = per_frame * (value / world) / 1e12
         traffic, traffic_detail = None, None
-        tp = os.path.join(ROOT, "profiles", "r2_traffic.json")
-        if os.path.exists(tp):
-            traffic_detail = json.load(open(tp))       # one representative tc_gemm launch from `ncu --set full`
-            traffic = traffic_detail.get("dram_bytes")  # dram__bytes_read.sum + dram__bytes_write.sum of that launch
-        roof = {"bound": "tensor", "kernel": "tc_gemm_kernel (tcgen05 implicit-GEMM conv / linear)",
+        roof = {"bound": "tensor", "kernel": "tc_gemm_kernel (wgmma implicit-GEMM conv / linear)",
                 "achieved": round(tc_tflops, 1), "peak": pk["tflops"], "unit": "TFLOP/s", "frac": round(tc_tflops / pk["tflops"], 4),
                 "traffic": traffic, "traffic_detail": traffic_detail, "peak_source": pk["src"],
                 "kernel_share_of_step": round(tc["ms"] / max(tot_ms, 1e-9), 4),
@@ -431,19 +470,19 @@ def main():
                                 "tflops": round(d["flops"] / max(d["ms"], 1e-9) / 1e9, 1),
                                 "gbs": round(d["bytes"] / max(d["ms"], 1e-9) / 1e6, 1)} for k, d in summ.items()}}
         line = {"metric": "latent-frames/sec", "value": round(value, 4), "unit": "latent-frames/s", "n_gpus": world,
-                "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": round(ms / args.steps, 2),
+                "steps": args.steps, "warmup": max(args.warmup, 1), "ms_per_step": round(ms / args.steps, 2),
                 "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "bf16" if ops.lib().gcd_act_dtype() == 1 else "f16",
                 "data": "synthetic (seeded random weights of the named architecture, random latents/conditioning)",
                 "config": {"workload": wl["name"], "clips_per_gpu_per_step": 1, "latent": [T_FRAMES, 4, LH, LW],
                            "sampler_steps": wl["steps"], "cfg_batch": 2 * T_FRAMES, "decode": not args.no_decode,
                            "parallelism": f"clips x{world} (one NCCL all_gather of latents per step)" if world > 1 else "single GPU",
-                           "l2": "no explicit flush: per-step working set (3.2 GB fp16 weights + multi-GB activations) >> 126 MB L2",
+                           "l2": "no explicit flush: per-step working set (3.2 GB fp16 weights + multi-GB activations) >> 50 MB L2",
                            "precision": "fp16 tensor-core operands, fp32 accumulate / residual stream / norms (UNet = the reference's fp16-autocast arithmetic; the VAE decode uses the same 16-bit operands where the reference decodes in fp32: 7.4e-4 rel-L2 at 576x1024)"},
                 "e2e": {"value": round(e2e_value, 4), "unit": "latent-frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                         "ms_per_step": round(ms_e2e / args.steps, 2),
                         "api": "gcd_b200.pipeline.GCDHotPath.sample_video(pinned host noise/cond) + frames -> pinned host"},
-                "gpu_launches": int(launches), "clocks": clk, "roofline": roof}
+                "gpu_launches": int(launches), "gpu": gpu_info(local), "clocks": clk, "roofline": roof}
         if extra:
             line["extra_workloads"] = extra
         if world == 1 and not args.no_cpu_baseline and not args.profile_run:

@@ -1,2 +1,2 @@
-"""gcd_b200 — B200-native (sm_100a) denoising hot path for Generative Camera Dolly (basilevh/gcd)."""
+"""gcd_b200 — H100-native (sm_90a) denoising hot path for Generative Camera Dolly (basilevh/gcd)."""
 __version__ = "0.1.0"

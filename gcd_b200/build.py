@@ -1,4 +1,4 @@
-"""Builds gcd_b200/libgcd_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds gcd_b200/libgcd_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m gcd_b200.build [--bf16] [--verbose]
 """
@@ -29,7 +29,7 @@ def build(force=False, bf16=False, verbose=False):
     os.makedirs(os.path.join(HERE, "build"), exist_ok=True)
     for src in SOURCES:
         obj = os.path.join(HERE, "build", src.replace(".cu", ".o"))
-        cmd = [nvcc, "-c", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3",
+        cmd = [nvcc, "-c", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
                "-std=c++17", "-o", obj, os.path.join(CSRC, src)]
         if bf16:
             cmd.insert(1, "-DGCD_ACT_BF16")

@@ -1,22 +1,15 @@
-// gcd_b200 — FlashAttention-style spatial self-attention for sm_100a, head_dim 64, tcgen05 + TMEM + TMA.
+// gcd_b200 — FlashAttention-style spatial self-attention for sm_90a, head_dim 64, wgmma + TMA.
 // Reference math: gcd-model/sgm/modules/attention.py:283-344 (CrossAttention.forward, context=None):
 //   out = softmax(q k^T / sqrt(64)) v, heads outer in the channel dim ("b n (h d) -> b h n d").
 //
-// One CTA per (128-query tile, head, frame); two CTAs co-reside per SM so one CTA's softmax overlaps the other's MMAs.
-//   warp 0    : TMA producer — K_j / V_j (64 keys each) through a 4-stage mbarrier ring (the only shared-memory operands).
-//   warp 1    : MMA issuer   — S_j = Q K_j^T  (M128 N64 K64, A = Q from TMEM, B = K K-major smem)        -> TMEM S[j&1]
-//                              O  += P_j V_j  (M128 N64 K64, A = P from TMEM, B = V MN-major smem)       -> TMEM O
-//   warp 2    : TMEM allocator (256 columns: S0 S1 O Q)
-//   warps 4.. : softmax — thread r owns query row r (SPLIT=2: two threads per row, 32 keys each): tcgen05.ld S row, online
-//               softmax in fp32 in the exp2 domain with packed f32x2 FMA/ADD and 3-input max; P_j is written back with
-//               tcgen05.st over the first half of S_j's own columns and consumed from there by the PV MMA, Q is loaded
-//               once from global memory into TMEM the same way. (v2 staged Q and P in shared memory: ncu showed the smem
-//               pipe ~75 % busy — 47 % tensor-core operand reads + 26 % P stores with 1.6x bank-conflict replays — as the
-//               co-limiter next to the MUFU pipe at 63 %.)
-//               O stays in TMEM: it is rescaled (tcgen05.ld / st) only when a row's running max grew by more than 2^8
-//               ("lazy rescale"); otherwise the stale max is kept, which is exact after the final 1/l normalisation.
-// Roofline note: per S element 256 tensor FLOPs vs one MUFU ex2 (16/clk/SM) -> MUFU-bound at ~half the bf16 peak
-// unless part of the exponentials is evaluated on the FMA pipe (EMU template parameter).
+// One CTA per (128-query tile, head, frame), three warpgroups:
+//   warpgroup 0    : TMA producer (one thread) — the CTA's Q tile once, then K_j / V_j (64 keys each) through a 4-stage
+//                    mbarrier ring, all 128B-swizzled.
+//   warpgroups 1, 2: 64 query rows each. Per key block: S = Q K_j^T (wgmma m64n64k16, both operands in shared memory,
+//                    fp32 S in registers); online softmax in the exp2 domain on the accumulator fragment (each row lives in
+//                    the 4 lanes of a quad); P is re-packed in registers as the 16-bit A operand of O += P V_j (wgmma with A
+//                    from registers, V as an MN-major B operand). While one warpgroup runs its softmax, the other's MMAs
+//                    keep the tensor cores busy.
 #include "common.cuh"
 #include "../../include/gcd_b200.h"
 #include <atomic>
@@ -26,15 +19,11 @@ using namespace ptx;
 namespace fa {
 constexpr int BQ = 128, BK = 64, D = 64;
 constexpr int KV_STAGES = 4;
-constexpr int KV_BYTES = BK * D * 2;         // 8 KB each for K and V
-constexpr int TM_S = 0, TM_O = 128, TM_Q = 192;   // TMEM columns: S[2] (P_j aliases the first 32 of S_j), O, Q (16-bit pairs)
-constexpr int X_BYTES = 2 * 2 * BQ * 4;     // row max / row sum exchange between the two threads of a row [parity][half][row]
-constexpr int SMEM = KV_STAGES * 2 * KV_BYTES + X_BYTES + 1024 + 256;
-constexpr float RESCALE_TAU = 8.0f;          // log2 units
+constexpr int TILE_BYTES = BK * D * 2;       // 8 KB: one 64-row x 64-channel box
+constexpr int SMEM = 2 * TILE_BYTES + KV_STAGES * 2 * TILE_BYTES + 256 + 1024;
 
 struct Params {
     int tokens, heads, nblk;
-    const act_t* qkv;
     act_t* out;
 };
 
@@ -43,294 +32,131 @@ __device__ __forceinline__ float ex2(float x) {
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-__device__ __forceinline__ float max3(float a, float b, float c) {
-    float d;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-    return d;
-}
-__device__ __forceinline__ uint64_t pk2(float a, float b) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-    return r;
-}
-__device__ __forceinline__ void upk2(uint64_t v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
-}
-__device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-    uint64_t d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-__device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
-    uint64_t d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-// 2^x for a pair on the FMA pipe: Cody-Waite split (round-to-nearest via the 1.5*2^23 trick) + degree-4 polynomial on
-// [-0.5, 0.5] (rel. err ~4e-6, far below the 16-bit P rounding), exponent inserted with integer adds.
-__device__ __forceinline__ uint64_t ex2_emu2(uint64_t x) {
-    const uint64_t MAGIC = pk2(12582912.0f, 12582912.0f), NMAGIC = pk2(-12582912.0f, -12582912.0f);
-    float x0, x1;
-    upk2(x, x0, x1);
-    x = pk2(fmaxf(x0, -126.0f), fmaxf(x1, -126.0f));
-    const uint64_t t = add2(x, MAGIC);                 // integer part in the low mantissa bits
-    const uint64_t n = add2(t, NMAGIC);                // rounded x
-    const uint64_t f = fma2(n, pk2(-1.0f, -1.0f), x);
-    uint64_t p = fma2(f, pk2(9.6181291e-3f, 9.6181291e-3f), pk2(5.5504109e-2f, 5.5504109e-2f));
-    p = fma2(p, f, pk2(2.4022651e-1f, 2.4022651e-1f));
-    p = fma2(p, f, pk2(6.9314718e-1f, 6.9314718e-1f));
-    p = fma2(p, f, pk2(1.0f, 1.0f));
-    float p0, p1, t0, t1;
-    upk2(p, p0, p1);
-    upk2(t, t0, t1);
-    p0 = __int_as_float(__float_as_int(p0) + (__float_as_int(t0) << 23));
-    p1 = __int_as_float(__float_as_int(p1) + (__float_as_int(t1) << 23));
-    return pk2(p0, p1);
-}
-template <int EMU, int SPLIT>
-__global__ void __launch_bounds__(128 + 128 * SPLIT, 2)
-attn_kernel(const __grid_constant__ CUtensorMap mapKV, const Params p) {
+
+__global__ void __launch_bounds__(384, 1)
+attn_kernel(const __grid_constant__ CUtensorMap mapQKV, const Params p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sK = smem;                                 // [stage][8 KB]
-    uint8_t* sV = sK + KV_STAGES * KV_BYTES;            // [stage][8 KB]
-    float* sx = reinterpret_cast<float*>(sV + KV_STAGES * KV_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KV_STAGES * KV_BYTES + X_BYTES);
-    uint64_t* q_full = bars;                   // Q rows stored to TMEM by the softmax threads
-    uint64_t* kv_full = bars + 1;              // KV_STAGES
-    uint64_t* kv_empty = kv_full + KV_STAGES;  // KV_STAGES
-    uint64_t* s_full = kv_empty + KV_STAGES;   // 2
-    uint64_t* p_full = s_full + 2;             // 2
-    uint64_t* pv_done = p_full + 2;            // 2: pv_done[j&1] completes a phase when P_j V_j has been accumulated into O
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + 2);
+    uint8_t* sQ = smem;                                 // [2 warpgroups][8 KB]
+    uint8_t* sK = sQ + 2 * TILE_BYTES;                  // [stage][8 KB]
+    uint8_t* sV = sK + KV_STAGES * TILE_BYTES;          // [stage][8 KB]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KV_STAGES * TILE_BYTES);
+    uint64_t* q_full = bars;
+    uint64_t* kv_full = bars + 1;                       // KV_STAGES
+    uint64_t* kv_empty = kv_full + KV_STAGES;           // KV_STAGES
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * BQ, head = blockIdx.y, frame = blockIdx.z;
     const int C = p.heads * D;
     const int nblk = p.nblk;
 
-    if (warp == 0 && lane == 0) prefetch_tmap(&mapKV);
-    if (warp == 1 && lane == 0) {
-        mbar_init(q_full, 128 * SPLIT);
-        for (int i = 0; i < KV_STAGES; i++) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
-        for (int i = 0; i < 2; i++) {
-            mbar_init(&s_full[i], 1); mbar_init(&p_full[i], 128 * SPLIT);
-            mbar_init(&pv_done[i], 1);
-        }
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&mapQKV);
+        mbar_init(q_full, 1);
+        for (int i = 0; i < KV_STAGES; i++) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 8); }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(tmem_slot, 256);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp < 4) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-        if (warp == 0 && lane == 0) {
-            // ------------------------------------------------ TMA producer
+        if (threadIdx.x == 0) {
+            // ------------------------------------------------ TMA producer (rows past `tokens` are zero-filled)
+            mbar_expect_tx(q_full, 2 * TILE_BYTES);
+            tma_load_3d(&mapQKV, sQ, q_full, head * D, q0, frame);
+            tma_load_3d(&mapQKV, sQ + TILE_BYTES, q_full, head * D, q0 + 64, frame);
             for (int j = 0; j < nblk; j++) {
                 const int s = j % KV_STAGES;
                 mbar_wait(&kv_empty[s], ((j / KV_STAGES) & 1) ^ 1);
-                mbar_expect_tx(&kv_full[s], 2 * KV_BYTES);
-                tma_load_3d(&mapKV, sK + s * KV_BYTES, &kv_full[s], C + head * D, j * BK, frame);
-                tma_load_3d(&mapKV, sV + s * KV_BYTES, &kv_full[s], 2 * C + head * D, j * BK, frame);
-            }
-        } else if (warp == 1 && lane == 0) {
-            // ------------------------------------------------ MMA issuer
-            constexpr uint32_t idesc_qk = make_idesc_f16(128, BK, 0, 0);   // A (TMEM), B K-major
-            constexpr uint32_t idesc_pv = make_idesc_f16(128, D, 0, 1);    // B (=V) MN-major
-            // tcgen05.mma executes in issue order: QK_{j+1} overwrites S[(j+1)&1] — which still holds P_{j-1} — only after
-            // PV_{j-1}, issued before it, has read it; and p_full(j-1) already implied that S_{j-1} had been consumed.
-            auto issue_qk = [&](int j) {
-                const int s = j % KV_STAGES;
-                mbar_wait(&kv_full[s], (j / KV_STAGES) & 1);
-                tc_fence_after();
-                const uint64_t kd = make_desc_sw128(smem_u32(sK + s * KV_BYTES), 16, 1024);
-#pragma unroll
-                for (int k = 0; k < 4; k++)
-                    umma_f16_ts(tmem_base + TM_S + (j & 1) * 64, tmem_base + TM_Q + k * 8, kd + (uint64_t)(k * 2), idesc_qk, k != 0);
-                umma_commit(&s_full[j & 1]);
-            };
-            mbar_wait(q_full, 0);
-            issue_qk(0);
-            for (int j = 0; j < nblk; j++) {
-                if (j + 1 < nblk) issue_qk(j + 1);
-                const int s = j % KV_STAGES;
-                mbar_wait(&p_full[j & 1], (j >> 1) & 1);      // P_j stored to TMEM and O rescaled if needed
-                tc_fence_after();
-                // V tile [64 keys][64 d]: MN-major B operand; 16 keys (2 groups of 8 rows, SBO=1024) per K step
-                const uint64_t vd = make_desc_sw128(smem_u32(sV + s * KV_BYTES), 1024, 1024);
-#pragma unroll
-                for (int k = 0; k < 4; k++)
-                    umma_f16_ts(tmem_base + TM_O, tmem_base + TM_S + (j & 1) * 64 + k * 8, vd + (uint64_t)(k * 128), idesc_pv,
-                                (j | k) != 0);
-                umma_commit(&pv_done[j & 1]);
-                umma_commit(&kv_empty[s]);
+                mbar_expect_tx(&kv_full[s], 2 * TILE_BYTES);
+                tma_load_3d(&mapQKV, sK + s * TILE_BYTES, &kv_full[s], C + head * D, j * BK, frame);
+                tma_load_3d(&mapQKV, sV + s * TILE_BYTES, &kv_full[s], 2 * C + head * D, j * BK, frame);
             }
         }
-    } else {
-        if (SPLIT == 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 200;");
-        else asm volatile("setmaxnreg.inc.sync.aligned.u32 96;");
-        // ---------------------------------------------------- softmax warps
-        // SPLIT threads share a query row (warps w and w+4 sit on the same TMEM lane quadrant): each owns NC of the block's 64
-        // key columns and the same NC of the 64 O columns; the row max (and at the end the row sum) is exchanged through smem.
-        constexpr int NC = BK / SPLIT;
-        const int q = warp & 3, half = (warp - 4) >> 2;
-        const int r = q * 32 + lane;
-        const int c0 = half * NC;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-        constexpr float SCALE_LOG2 = 0.125f * 1.4426950408889634f;
-        const uint64_t SC2 = pk2(SCALE_LOG2, SCALE_LOG2);
-        float m_run = -INFINITY, l_run = 0.f;
-        {
-            // my (part of the) Q row: global -> registers -> TMEM (two 16-bit values per column = the MMA's A operand layout)
-            uint32_t qv[NC / 2];
-            const uint4* src = reinterpret_cast<const uint4*>(p.qkv + ((int64_t)frame * p.tokens + q0 + r) * 3 * C + head * D + c0);
-            const bool qvalid = q0 + r < p.tokens;
-#pragma unroll
-            for (int i = 0; i < NC / 8; i++) {
-                const uint4 t = qvalid ? __ldg(src + i) : make_uint4(0, 0, 0, 0);
-                qv[4 * i] = t.x; qv[4 * i + 1] = t.y; qv[4 * i + 2] = t.z; qv[4 * i + 3] = t.w;
-            }
-            if constexpr (SPLIT == 1) tmem_st32(lane_addr + TM_Q, qv);
-            else tmem_st16(lane_addr + TM_Q + half * 16, qv);
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(q_full);
-        }
-
-        for (int j = 0; j < nblk; j++) {
-            mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-            tc_fence_after();
-            uint32_t sv[NC];
-#pragma unroll
-            for (int h2 = 0; h2 < NC / 32; h2++)
-                tmem_ld32(lane_addr + TM_S + (j & 1) * 64 + c0 + h2 * 32, *reinterpret_cast<uint32_t(*)[32]>(&sv[h2 * 32]));
-            tmem_ld_wait();
-
-            const int kv_left = p.tokens - j * BK - c0;   // valid keys among my columns
-            if (kv_left < NC) {
-#pragma unroll
-                for (int i = 0; i < NC; i++)
-                    if (i >= kv_left) sv[i] = __float_as_uint(-INFINITY);
-            }
-            // row max: independent 3-input-max chains of 16 values (a single chain would be 32 dependent FMNMX3 long)
-            float mq[NC / 16];
-#pragma unroll
-            for (int c = 0; c < NC / 16; c++) {
-                const int b = c * 16;
-                mq[c] = max3(__uint_as_float(sv[b]), __uint_as_float(sv[b + 1]), __uint_as_float(sv[b + 2]));
-#pragma unroll
-                for (int i = 3; i + 1 < 16; i += 2) mq[c] = max3(mq[c], __uint_as_float(sv[b + i]), __uint_as_float(sv[b + i + 1]));
-                mq[c] = fmaxf(mq[c], __uint_as_float(sv[b + 15]));
-            }
-            float mx = fmaxf(mq[0], mq[1]);
-            if (NC == 64) mx = max3(mx, mq[NC / 16 - 2], mq[NC / 16 - 1]);
-            if (SPLIT == 2) {
-                sx[((j & 1) * 2 + half) * BQ + r] = mx;
-                named_bar_sync(1 + q, 64);
-                mx = fmaxf(mx, sx[((j & 1) * 2 + (half ^ 1)) * BQ + r]);
-            }
-            const float m_new = fmaxf(m_run, mx * SCALE_LOG2);
-
-            if (j > 0) {
-                if (__any_sync(0xffffffffu, m_new - m_run > RESCALE_TAU)) {
-                    // O must hold blocks 0..j-1 before it is rescaled: only this (rare) path waits for the previous PV.
-                    mbar_wait(&pv_done[(j - 1) & 1], ((j - 1) >> 1) & 1);
-                    tc_fence_after();
-                    const float alpha = ex2(m_run - m_new);
-                    const uint64_t A2 = pk2(alpha, alpha);
-#pragma unroll
-                    for (int hlf = 0; hlf < NC / 32; hlf++) {
-                        uint32_t v[32];
-                        tmem_ld32(lane_addr + TM_O + c0 + hlf * 32, v);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 32; i += 2) {
-                            float a, b;
-                            upk2(mul2(pk2(__uint_as_float(v[i]), __uint_as_float(v[i + 1])), A2), a, b);
-                            v[i] = __float_as_uint(a); v[i + 1] = __float_as_uint(b);
-                        }
-                        tmem_st32(lane_addr + TM_O + c0 + hlf * 32, v);
-                    }
-                    tmem_st_wait();
-                    tc_fence_before();
-                    l_run *= alpha;
-                    m_run = m_new;
-                }
-            } else {
-                m_run = m_new;
-            }
-            // p = 2^(s*scale - m_run), row sum, P row (packed 16-bit pairs) -> TMEM over my own S columns
-            const uint64_t NM2 = pk2(-m_run, -m_run);
-            uint64_t lsum2 = pk2(0.f, 0.f);
-            uint32_t pw[NC / 2];
-#pragma unroll
-            for (int i = 0; i < NC / 2; i++) {
-                const uint64_t x = fma2(pk2(__uint_as_float(sv[2 * i]), __uint_as_float(sv[2 * i + 1])), SC2, NM2);
-                uint64_t pe;
-                if (EMU > 0 && (i % (EMU > 0 ? EMU : 1)) == 0) {
-                    pe = ex2_emu2(x);
-                } else {
-                    float x0, x1;
-                    upk2(x, x0, x1);
-                    pe = pk2(ex2(x0), ex2(x1));
-                }
-                lsum2 = add2(lsum2, pe);
-                float p0, p1;
-                upk2(pe, p0, p1);
-                pw[i] = pack2(p0, p1);
-            }
-            // all threads of the row have finished reading S_j (SPLIT=2: the exchange barrier above ordered the partner's
-            // tcgen05.ld before this store), so P_j may overwrite columns [0,32) of S_j
-            if constexpr (SPLIT == 1) tmem_st32(lane_addr + TM_S + (j & 1) * 64, pw);
-            else tmem_st16(lane_addr + TM_S + (j & 1) * 64 + half * 16, pw);
-            {
-                float a, b;
-                upk2(lsum2, a, b);
-                l_run += a + b;
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&p_full[j & 1]);
-        }
-        // ---- epilogue: O / l
-        if (SPLIT == 2) {
-            // buffer (nblk&1) was last read in block nblk-2, before both warps passed the exchange barrier of block nblk-1
-            sx[((nblk & 1) * 2 + half) * BQ + r] = l_run;
-            named_bar_sync(1 + q, 64);
-            l_run += sx[((nblk & 1) * 2 + (half ^ 1)) * BQ + r];
-        }
-        mbar_wait(&pv_done[(nblk - 1) & 1], ((nblk - 1) >> 1) & 1);
-        tc_fence_after();
-        const float inv = 1.0f / l_run;
-        const bool valid = q0 + r < p.tokens;
-        uint4* dst = reinterpret_cast<uint4*>(p.out + ((int64_t)frame * p.tokens + q0 + r) * C + head * D + c0);
-#pragma unroll
-        for (int hlf = 0; hlf < NC / 32; hlf++) {
-            uint32_t v[32];
-            tmem_ld32(lane_addr + TM_O + c0 + hlf * 32, v);
-            tmem_ld_wait();
-            if (valid) {
-#pragma unroll
-                for (int c = 0; c < 4; c++)
-                    dst[hlf * 4 + c] = make_uint4(
-                        pack2(__uint_as_float(v[c * 8 + 0]) * inv, __uint_as_float(v[c * 8 + 1]) * inv),
-                        pack2(__uint_as_float(v[c * 8 + 2]) * inv, __uint_as_float(v[c * 8 + 3]) * inv),
-                        pack2(__uint_as_float(v[c * 8 + 4]) * inv, __uint_as_float(v[c * 8 + 5]) * inv),
-                        pack2(__uint_as_float(v[c * 8 + 6]) * inv, __uint_as_float(v[c * 8 + 7]) * inv));
-            }
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 256);
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // ---------------------------------------------------- consumers: 64 query rows per warpgroup
+    const int cw = (warp >> 2) - 1;
+    const int r0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);    // tile row of this thread's first accumulator row (+8: second)
+    const int cb = 2 * (lane & 3);
+    constexpr float SCALE_LOG2 = 0.125f * 1.4426950408889634f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; i++) o[i] = 0.f;
+    const uint64_t qd = make_desc_sw128(smem_u32(sQ + cw * TILE_BYTES), 16, 1024);
+    mbar_wait(q_full, 0);
+
+    for (int j = 0; j < nblk; j++) {
+        const int s = j % KV_STAGES;
+        mbar_wait(&kv_full[s], (j / KV_STAGES) & 1);
+        // S = Q K_j^T: K tile [64 keys][64 d] is the K-major B operand
+        float sv[32];
+        const uint64_t kd = make_desc_sw128(smem_u32(sK + s * TILE_BYTES), 16, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; k++) wgmma_m64n64_ss(sv, qd + 2 * k, kd + 2 * k, k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(sv);
+
+        const int kv_left = p.tokens - j * BK;           // valid keys in this block
+        if (kv_left < BK) {
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                if (8 * i + cb >= kv_left) { sv[4 * i] = -INFINITY; sv[4 * i + 2] = -INFINITY; }
+                if (8 * i + cb + 1 >= kv_left) { sv[4 * i + 1] = -INFINITY; sv[4 * i + 3] = -INFINITY; }
+            }
+        }
+        uint32_t pa[4][4];                               // P as the A operand of the four K=16 steps of P V_j
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            float mx = -INFINITY;
+#pragma unroll
+            for (int i = 0; i < 8; i++) mx = fmaxf(mx, fmaxf(sv[4 * i + 2 * h], sv[4 * i + 2 * h + 1]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float m_new = fmaxf(m_run[h], mx * SCALE_LOG2);
+            const float alpha = ex2(m_run[h] - m_new);   // 0 on the first block (m_run = -inf)
+            m_run[h] = m_new;
+            float ls = 0.f;
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const float e0 = ex2(fmaf(sv[4 * i + 2 * h], SCALE_LOG2, -m_new));
+                const float e1 = ex2(fmaf(sv[4 * i + 2 * h + 1], SCALE_LOG2, -m_new));
+                ls += e0 + e1;
+                // accumulator columns 8i..8i+7 = A columns 8(i&1).. of K step i>>1; register 2(i&1) + h
+                pa[i >> 1][2 * (i & 1) + h] = pack2(e0, e1);
+                o[4 * i + 2 * h] *= alpha;
+                o[4 * i + 2 * h + 1] *= alpha;
+            }
+            l_run[h] = l_run[h] * alpha + ls;
+        }
+        // O += P V_j: V tile [64 keys][64 d] is an MN-major B operand; a K step of 16 keys = 2048 bytes
+        const uint64_t vd = make_desc_sw128(smem_u32(sV + s * TILE_BYTES), 1024, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; k++) wgmma_m64n64_rs_tb(o, pa[k], vd + (uint64_t)(k * 128));
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(o);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&kv_empty[s]);
+    }
+    // ---- epilogue: O / l (row sums completed over the quad)
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        float l = l_run[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = 1.0f / l;
+        const int row = q0 + r0 + 8 * h;
+        if (row >= p.tokens) continue;
+        act_t* dst = p.out + ((int64_t)frame * p.tokens + row) * C + head * D + cb;
+#pragma unroll
+        for (int i = 0; i < 8; i++)
+            *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
     }
 }
 }  // namespace fa
@@ -338,36 +164,22 @@ attn_kernel(const __grid_constant__ CUtensorMap mapKV, const Params p) {
 extern "C" int gcd_attention_spatial(const void* qkv, int frames, int tokens, int heads, void* out, void* stream) {
     GCD_REQUIRE(qkv && out && frames > 0 && tokens > 0 && heads > 0, "attention_spatial: bad arguments");
     GCD_REQUIRE(frames <= 65535 && heads <= 65535, "attention_spatial: grid too large");
-    static int emu_env = -2, split = 1;
-    if (emu_env == -2) {
-#define FA_CFG(E, S) GCD_CUDA_CHECK(cudaFuncSetAttribute(fa::attn_kernel<E, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, fa::SMEM))
-        FA_CFG(0, 1); FA_CFG(4, 1); FA_CFG(0, 2); FA_CFG(4, 2);
-#undef FA_CFG
-        const char* e = getenv("GCD_FA_EMU");            // experiments: share of exponentials on the FMA pipe: 0 or 4 (25 %)
-        const char* sp = getenv("GCD_FA_SPLIT");         // experiments: threads per query row; 2 measured 10 % slower
-        split = (sp && atoi(sp) == 2) ? 2 : 1;
-        emu_env = e ? (atoi(e) == 4 ? 4 : 0) : -1;
+    static bool configured = false;
+    if (!configured) {
+        GCD_CUDA_CHECK(cudaFuncSetAttribute(fa::attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, fa::SMEM));
+        configured = true;
     }
-    // Moving every 4th exponential pair to the FMA pipe gains ~1-2 % on the 9216-token level in a short burst at 1.9 GHz
-    // (tools/bench_attn.py) but LOSES 1.2 % sustained under the power cap the real step runs at (tools/bench_sustained.py: 742 vs
-    // 751 TFLOP/s, 1687 vs 1755 MHz at the same 991 W — the polynomial costs more energy than the MUFU): off by default.
-    const int emu = emu_env >= 0 ? emu_env : 0;
-    (void)tokens;
     const int C = heads * 64;
-    CUtensorMap mKV;
+    CUtensorMap mQKV;
     uint64_t dims[3] = {(uint64_t)3 * C, (uint64_t)tokens, (uint64_t)frames};
     uint64_t str[2] = {(uint64_t)3 * C * 2, (uint64_t)tokens * 3 * C * 2};
-    uint32_t boxk[3] = {64, fa::BK, 1};
-    int rc = gcd_make_tmap(&mKV, qkv, 3, dims, str, boxk, nullptr, 128, 0);
+    uint32_t box[3] = {64, 64, 1};
+    int rc = gcd_make_tmap(&mQKV, qkv, 3, dims, str, box, nullptr, 128, 0);
     if (rc) return rc;
     fa::Params p;
-    p.tokens = tokens; p.heads = heads; p.nblk = (tokens + fa::BK - 1) / fa::BK; p.qkv = (const act_t*)qkv; p.out = (act_t*)out;
+    p.tokens = tokens; p.heads = heads; p.nblk = (tokens + fa::BK - 1) / fa::BK; p.out = (act_t*)out;
     dim3 grid((tokens + fa::BQ - 1) / fa::BQ, heads, frames);
-    cudaStream_t st = (cudaStream_t)stream;
-#define FA_GO(E, S) fa::attn_kernel<E, S><<<grid, 128 + 128 * S, fa::SMEM, st>>>(mKV, p)
-    if (split == 1) { if (emu == 4) FA_GO(4, 1); else FA_GO(0, 1); }
-    else { if (emu == 4) FA_GO(4, 2); else FA_GO(0, 2); }
-#undef FA_GO
+    fa::attn_kernel<<<grid, 384, fa::SMEM, (cudaStream_t)stream>>>(mQKV, p);
     GCD_CUDA_CHECK(cudaGetLastError());
     g_launches++;
     return 0;

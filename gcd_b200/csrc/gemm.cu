@@ -1,21 +1,7 @@
-// gcd_b200 — tcgen05 implicit-GEMM kernel (Linear / Conv2d 3x3 & 1x1 / Conv3d (3,1,1) / batched matmul).
+// gcd_b200 — wgmma implicit-GEMM kernel for sm_90a (Linear / Conv2d 3x3 & 1x1 / Conv3d (3,1,1) / batched matmul).
 //
-// One persistent, warp-specialised kernel per output-tile width BN in {128,160,256}:
-//   warp 0   : TMA producer  — per (tap, 64-channel chunk): one 4-D box of the channels-last activation tensor
-//              (out-of-range coordinates zero-filled by TMA = conv zero padding) + one 3-D box of the weights,
-//              both landing 128B-swizzled in shared memory, signalled on an mbarrier ring.
-//   warp 1   : MMA issuer    — a single thread issues tcgen05.mma (M=128, N=BN, K=16, fp32 accumulate in TMEM),
-//              tcgen05.commit frees smem stages and publishes the accumulator.
-//   warp 2   : TMEM allocator (512 columns = 2 accumulator stages so the epilogue overlaps the next tile's MMAs).
-//   warps 4.. : epilogue     — NWG warpgroups (2 by default); the 128-byte-row column spans of the CTA's tile stream are dealt
-//              round-robin to them; per 32-column chunk: tcgen05.ld the accumulator row of each thread, fused bias (+ per-frame
-//              vector) / SiLU / GEGLU / residual blend on packed fp32 pairs, then a swizzled smem staging tile that one thread
-//              hands to the TMA store engine (cp.async.bulk.tensor ... bulk_group). Residual tiles are prefetched one chunk
-//              ahead by TMA loads into swizzled smem. No per-thread global loads/stores of activations, no bounds checks
-//              (TMA clips), compact code (the first register-transposed epilogue was instruction-cache bound:
-//              profiles/r1_notes.md §1).
-// Cluster modes (template MODE): 1 single CTA; 2 weight tile TMA-multicast across a CTA pair; 3 CTA-pair MMA
-// (tcgen05.mma.cta_group::2, M = 256); 4 = 3 with both 160-column halves of an N = 320 row block fed from one activation tile.
+// acc[r, n] = sum_{tap, c} A[(x,y,z)(r) * in_mul + tap_off(tap), c] * W[n, tap*C + c], fp16/bf16 operands, fp32 accumulate,
+// with the whole epilogue (bias, per-row vector, SiLU, scale, GEGLU, residual blends, GroupNorm statistics) fused.
 // Replaces cuDNN/cuBLAS calls behind nn.Conv2d / nn.Conv3d / nn.Linear in
 //   gcd-model/sgm/modules/diffusionmodules/openaimodel.py:213-357 (ResBlock), :110-210 (Up/Downsample),
 //   gcd-model/sgm/modules/attention.py:87-113,255-344 (FeedForward/GEGLU, CrossAttention projections),
@@ -101,531 +87,271 @@ struct TcParams {
     int8_t tdx[9], tdy[9], tdz[9];
     int N, n_tiles;
     int w_batched;
-    int stages;                 // smem ring depth (runtime: depends on which epilogue staging buffers are needed)
-    int obufs;                  // output staging tiles per epilogue warpgroup (2 when the K loop is short)
-    int rbufs;                  // residual tiles in flight per epilogue warpgroup (2 when the K loop is short: HBM-latency bound)
+    int stages;                 // smem ring depth
     // epilogue
     const float* bias;
     const float* rowvec;
     int rpv, ldv;
-    int has_r1, has_r2, r1f32, r2f32;
+    const void* res1;
+    const void* res2;
+    int ld1, ld2, r1f32, r2f32;
     float a0, a1, a2;
-    int of32, geglu, act;
+    void* out;
+    int ldo, of32, geglu, act;
     double* gn_stats;           // fused GroupNorm statistics of the output (nullptr: off)
     int gn_cpg, gn_groups;
-    int gn_acc;                 // 1: accumulate the statistics per CTA in smem across tiles, flush when the image changes
     long long gn_rpi;
 };
 
-constexpr int TC_A_BYTES = 128 * 128;
-constexpr int TC_SMEM_MAX = 232448;           // 227 KB opt-in maximum per CTA
+constexpr int TC_A_BYTES = 128 * 128;          // one 128-row x 64-channel activation box, 128B-swizzled
+constexpr int TC_SMEM_MAX = 232448;            // 227 KB opt-in maximum per CTA
+constexpr int TC_THREADS = 384;                // producer warpgroup + two consumer warpgroups
 
-__device__ __forceinline__ uint4 ld_shared_v4(const uint8_t* p) { return *reinterpret_cast<const uint4*>(p); }
-
-// Row r of a swizzled staging tile whose rows are `nch` 16-byte chunks wide (8: SW128, 4: SW64, 2: SW32):
-// byte offset of logical chunk c  (Swizzle<B,4,3> with B = log2(nch); sh = 3 - B).
-__device__ __forceinline__ uint32_t stg_off(int r, int c, int nch, int sh) {
-    return (uint32_t)(r * nch + (c ^ ((r >> sh) & (nch - 1)))) << 4;
+// residuals: plain loads (the output may alias a residual: each element is read, then written, by the same thread)
+__device__ __forceinline__ float ld_res(const void* base, bool f32, int64_t off) {
+    return f32 ? reinterpret_cast<const float*>(base)[off] : act2f(reinterpret_cast<const act_t*>(base)[off]);
+}
+__device__ __forceinline__ float2 ld_res2(const void* base, bool f32, int64_t off) {
+    if (f32) return *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(base) + off);
+    return unpack2(*reinterpret_cast<const uint32_t*>(reinterpret_cast<const act_t*>(base) + off));
 }
 
-// x[0..32) += a * (row r of a swizzled residual tile holding 32 columns, float32 or act)
-__device__ __forceinline__ void add_residual_row(float* xf, const uint8_t* base, int r, bool f32, float a) {
-    if (f32) {
-#pragma unroll
-        for (int c = 0; c < 8; c++) {
-            const uint4 t = ld_shared_v4(base + stg_off(r, c, 8, 0));
-            xf[4 * c] += a * __uint_as_float(t.x); xf[4 * c + 1] += a * __uint_as_float(t.y);
-            xf[4 * c + 2] += a * __uint_as_float(t.z); xf[4 * c + 3] += a * __uint_as_float(t.w);
-        }
-    } else {
-#pragma unroll
-        for (int c = 0; c < 4; c++) {
-            const uint4 t = ld_shared_v4(base + stg_off(r, c, 4, 1));
-            float2 f;
-            f = unpack2(t.x); xf[8 * c] += a * f.x; xf[8 * c + 1] += a * f.y;
-            f = unpack2(t.y); xf[8 * c + 2] += a * f.x; xf[8 * c + 3] += a * f.y;
-            f = unpack2(t.z); xf[8 * c + 4] += a * f.x; xf[8 * c + 5] += a * f.y;
-            f = unpack2(t.w); xf[8 * c + 6] += a * f.x; xf[8 * c + 7] += a * f.y;
-        }
-    }
-}
-
-// MODE 1: one CTA per tile. MODE 2: 2-CTA cluster on adjacent M-tiles of one N-tile; each CTA loads half of the weight
-// tile and TMA-multicasts it into both CTAs' shared memory (halves the L2 -> SM weight traffic; the level-1 convs / K=320
-// GEMMs were bound by it: profiles/r1_ncu_prof_conv.txt, lts 62 %); MMAs stay 1-CTA. MODE 3: CTA pair with
-// tcgen05.mma.cta_group::2 — ONE M=256 MMA per pair issued by the leader CTA, each CTA keeps only its half of the weight
-// tile in smem (also halves the smem operand reads per FLOP: a 1-CTA M128xN160 MMA needs 115 of the 128 B/clk).
-// KC = 64-wide K chunks per pipeline stage: 2 for narrow tiles (BN <= 160), whose 4 MMAs per chunk (320 cycles) are
-// shorter than the issuing thread's per-stage overhead (mbarrier wait + fence + commit) — measured: BN=160 tiles
-// plateaued at 1.12 PFLOP/s in every mode while BN=256 reached 1.45-1.54 (tools/bench_convgemm.py).
-// NWG = epilogue warpgroups (2 or 3; 128 + 128*NWG threads). The accumulator column SPANS of the tile stream are dealt
-// round-robin to the warpgroups ACROSS tiles (span number G_k + s of the CTA's k-th tile goes to warpgroup (G_k + s) % NWG), so
-// every warpgroup stays busy whatever the number of spans per tile (GEGLU tiles have two). ncu on the K=320 GEGLU GEMM
-// (profiles/r2_notes.md §1): issue slots 46 %, tensor pipe 40 %, each epilogue warp issuing only 20 % of the time (fixed-latency
-// dependency stalls) — the epilogue was latency-bound with two warps per scheduler; NWG = 3 puts three there. With NWG = 3 the
-// register file is re-split with setmaxnreg (producer / MMA / allocator warps 56, epilogue warps 152).
-template <int BN, int MODE, int KC, int NWG>
-__global__ void __launch_bounds__(128 + 128 * NWG, 1)
-tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-               const __grid_constant__ CUtensorMap mapO, const __grid_constant__ CUtensorMap mapO2,
-               const __grid_constant__ CUtensorMap mapR1, const __grid_constant__ CUtensorMap mapR2, const TcParams p) {
-    constexpr int CL = MODE >= 2 ? 2 : 1;
-    constexpr bool PAIR = MODE >= 3;
-    // MODE 4 (WIDE, N == 2*BN == 320): one mainloop pass feeds BOTH N-halves — every activation tile that lands in shared memory
-    // is used by two MMAs (the two weight halves sit side by side in the stage), i.e. a 256 x 320 tile per CTA pair: 36 KB of
-    // operands per 64-wide K chunk instead of 2 x 26 KB (-31 % L2 -> SM traffic; the N = 320 convs are bound by it and, in the
-    // power-capped step, by the energy it costs: profiles/r2_notes.md §7). The accumulators rotate through three 160-column TMEM
-    // regions: virtual tile v (= 2*pass + half) lives in region v % 3, so pass p+1 needs the region of (pass p, half 0) back —
-    // the epilogue of the second half overlaps the next pass.
-    constexpr bool WIDE = MODE == 4;
-    static_assert(!WIDE || (BN == 160 && KC == 1), "wide mode: two 160-column halves, K = 64 stages");
-    constexpr int B_BYTES = (PAIR ? BN * 64 : BN * 128) * (WIDE ? 2 : 1);     // weight bytes held per CTA and 64-wide K chunk
+// One persistent, warp-specialised CTA per SM; the 128-row M-tile is a TW x TH x TN box of output positions.
+//   warpgroup 0 : TMA producer (one thread) — per (tap, 64-channel chunk): one 4-D box of the channels-last activation
+//                 tensor (out-of-range coordinates zero-filled by TMA = conv zero padding) + one 3-D box of BN weight rows,
+//                 both landing 128B-swizzled in shared memory, signalled on an mbarrier ring. It runs ahead into the next
+//                 tile while the consumers are in their epilogue.
+//   warpgroups 1, 2 : consumers — rows [64*(wg-1), +64) of the tile: wgmma m64nBNk16 (fp32 accumulators in registers, one
+//                 batch in flight while the previous stage is released), then the fused epilogue straight from the
+//                 accumulator registers: bias (+ per-row vector) / SiLU / scale / GEGLU / two residual blends, 16-bit or fp32
+//                 stores, and the GroupNorm statistics of the stored values.
+template <int BN>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const TcParams p) {
+    constexpr int B_BYTES = BN * 128;
+    constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES;
+    constexpr int NACC = BN / 2;
     extern __shared__ __align__(1024) uint8_t smem[];     // SWIZZLE_128B tiles need 1024-byte alignment
     if ((smem_u32(smem) & 1023u) != 0) __trap();
     const int STAGES = p.stages;
-    uint8_t* sA = smem;                                    // [STAGES][KC][16 KB]
-    uint8_t* sB = sA + STAGES * KC * TC_A_BYTES;           // [STAGES][KC][B_BYTES]
-    const int OT = 16384;                                             // bytes of one output staging tile (128 x 128 B)
-    const int RT1 = p.has_r1 ? (p.r1f32 ? 16384 : 8192) : 0, RT2 = p.has_r2 ? (p.r2f32 ? 16384 : 8192) : 0;
-    uint8_t* sO = sB + STAGES * KC * B_BYTES;               // [NWG warpgroups][obufs] output staging
-    uint8_t* sR1 = sO + NWG * p.obufs * OT;                 // [NWG warpgroups][rbufs] residual 1 (if any)
-    uint8_t* sR2 = sR1 + NWG * p.rbufs * RT1;               // [NWG warpgroups][rbufs] residual 2 (if any)
-    float* sBias = reinterpret_cast<float*>(sR2 + NWG * p.rbufs * RT2); // [NWG][256] bias slice of the current tile, per warpgroup
-    float* sStat = sBias + NWG * 256;       // [4*NWG epilogue warps][32 groups][sum, sum of squares] (gn_acc only)
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sStat + (p.gn_acc ? NWG * 256 : 0));
+    float* sStat = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);     // [8 consumer warps][BN][sum, sum of squares]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sStat + (p.gn_stats ? 8 * BN * 2 : 0));
     uint64_t* full = bars;                 // [STAGES]
     uint64_t* empty = bars + 8;            // [STAGES]  (STAGES <= 8)
-    uint64_t* tfull = bars + 16;           // [2]
-    uint64_t* tempty = bars + 18;          // [2]  (WIDE: [3], one per TMEM region)
-    uint64_t* rfull = bars + 21;           // [NWG warpgroups][2] residual tiles landed
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 21 + 2 * NWG);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         prefetch_tmap(&mapA);
         prefetch_tmap(&mapB);
-        prefetch_tmap(&mapO);
-    }
-    const uint32_t crank = (CL == 2) ? cluster_ctarank() : 0u;
-    if (warp == 1 && lane == 0) {
         for (int i = 0; i < STAGES; i++) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], MODE == 2 ? 2 : 1);   // MODE 2: a multicast stage is free once BOTH CTAs' MMAs drained it
+            mbar_init(&empty[i], 8);       // one arrival per consumer warp
         }
-        for (int i = 0; i < 2; i++) mbar_init(&tfull[i], 1);
-        for (int i = 0; i < 3; i++) mbar_init(&tempty[i], (PAIR ? 2 : 1) * 128 * NWG);   // PAIR: the leader's MMA waits for both CTAs' epilogues
-        for (int i = 0; i < 2 * NWG; i++) mbar_init(&rfull[i], 1);
         fence_barrier_init();
     }
-    if (warp == 2) { if (PAIR) tmem_alloc_2cta(tmem_slot, 512); else tmem_alloc(tmem_slot, 512); }
-    tc_fence_before();
-    if (CL == 2) cluster_sync_all(); else __syncthreads();     // barrier inits visible cluster-wide before any remote arrive
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
 
-    // Persistent schedule over (M-tile group, N-tile): a cluster takes CL adjacent M-tiles of one N-tile. `tile` below is
-    // a group index; mt may point one past the last M-tile (phantom tile: all loads zero-fill, all stores are clipped).
     const int m_tiles = p.ntx * p.nty * p.ntz;
-    const int total = ((m_tiles + CL - 1) / CL) * p.n_tiles;
-    const int tile0 = blockIdx.x / CL, tile_step = gridDim.x / CL;
-    // i-th tile of this cluster. WIDE: the mainloop walks M-groups (passes); the epilogue sees virtual tiles (group, half) =
-    // tile index 2*group + half, both halves of a group consecutively on the same cluster.
-    auto tile_at = [&](int i) { return WIDE ? 2 * (tile0 + (i >> 1) * tile_step) + (i & 1) : tile0 + i * tile_step; };
+    const int total = m_tiles * p.n_tiles;
     const int kiters = p.ntaps * p.kchunks;
     const int TW = 1 << p.lTW, TH = 1 << p.lTH;
     const int TN = 128 >> (p.lTW + p.lTH);
 
     if (warp < 4) {
-    // NWG == 3 (512 threads): 4 x 32 x 56 + 12 x 32 x 152 = 65 536 registers. Each role's code sits in the same branch as its
-    // setmaxnreg so that ptxas allocates that region against the new limit.
-    if (NWG == 3) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-    if (warp == 0) {
-        if (lane == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (threadIdx.x == 0) {
             // ===================== TMA producer =====================
             int stage = 0;
             uint32_t phase = 0;
-            // WIDE: one pass per M-group (both N-halves); otherwise one pass per tile
-            for (int pi = 0;; pi++) {
-                const int tile = WIDE ? tile_at(2 * pi) : tile_at(pi);
-                if (tile >= total) break;
-                const int nt = WIDE ? 0 : tile % p.n_tiles;
-                const int mt = (tile / p.n_tiles) * CL + crank;
+            for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+                const int nt = tile % p.n_tiles;
+                const int mt = tile / p.n_tiles;
                 const int tx = mt % p.ntx;
                 const int ty = (mt / p.ntx) % p.nty;
                 const int tz = mt / (p.ntx * p.nty);
                 const int x0 = tx * TW * p.in_mul, y0 = ty * TH * p.in_mul, z0 = tz * TN;
                 const int wy = p.w_batched ? ty : 0;
-                const int ntile_w = min(BN, ((p.N - nt * BN) + 15) & ~15);     // width of this N-tile (see MMA issuer)
-                // flattened (tap, channel-chunk) sequence, KC chunks per stage
-                for (int q0 = 0; q0 < kiters; q0 += KC) {
-                    const int nch = min(KC, kiters - q0);
+                for (int q = 0; q < kiters; q++) {
+                    const int tap = q / p.kchunks, kc = q - tap * p.kchunks;
                     mbar_wait(&empty[stage], phase ^ 1);
-                    if (PAIR) { if (crank == 0) mbar_expect_tx(&full[stage], 2 * nch * (TC_A_BYTES + B_BYTES)); }
-                    else mbar_expect_tx(&full[stage], nch * (TC_A_BYTES + B_BYTES));
-                    for (int c = 0; c < nch; c++) {
-                        const int qq = q0 + c;
-                        const int tap = qq / p.kchunks, kc = qq - tap * p.kchunks;
-                        const int cx = x0 + p.tdx[tap], cy = y0 + p.tdy[tap], cz = z0 + p.tdz[tap];
-                        uint8_t* dA = sA + (stage * KC + c) * TC_A_BYTES;
-                        uint8_t* dB = sB + (stage * KC + c) * B_BYTES;
-                        if (WIDE) {        // my 80 weight rows of each N-half, side by side
-                            tma_load_4d_2sm(&mapA, dA, &full[stage], kc * 64, cx, cy, cz);
-                            tma_load_3d_2sm(&mapB, dB, &full[stage], qq * 64, crank * (BN / 2), wy);
-                            tma_load_3d_2sm(&mapB, dB + B_BYTES / 2, &full[stage], qq * 64, BN + crank * (BN / 2), wy);
-                        } else if (PAIR) { // both CTAs' bytes are reported to the leader's barrier
-                            tma_load_4d_2sm(&mapA, dA, &full[stage], kc * 64, cx, cy, cz);
-                            tma_load_3d_2sm(&mapB, dB, &full[stage], qq * 64, nt * BN + crank * (ntile_w / 2), wy);
-                        } else {
-                            tma_load_4d(&mapA, dA, &full[stage], kc * 64, cx, cy, cz);
-                            if (CL == 2)   // my half of the weight tile -> both CTAs
-                                tma_load_3d_mc(&mapB, dB + crank * (B_BYTES / 2), &full[stage], qq * 64,
-                                               nt * BN + crank * (BN / 2), wy, (uint16_t)0x3);
-                            else
-                                tma_load_3d(&mapB, dB, &full[stage], qq * 64, nt * BN, wy);
-                        }
-                    }
+                    mbar_expect_tx(&full[stage], STAGE_BYTES);
+                    uint8_t* dA = smem + stage * STAGE_BYTES;
+                    tma_load_4d(&mapA, dA, &full[stage], kc * 64, x0 + p.tdx[tap], y0 + p.tdy[tap], z0 + p.tdz[tap]);
+                    tma_load_3d(&mapB, dA + TC_A_BYTES, &full[stage], q * 64, nt * BN, wy);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && !(PAIR && crank != 0)) {
-            // ===================== MMA issuer (PAIR: leader CTA only) =====================
-            // the last N-tile of a row may be narrower than BN: issue its MMAs with the actual width (multiple of 16)
-            int stage = 0;
-            uint32_t phase = 0;
-            int it = 0;
-            for (;; it++) {
-                const int tile = WIDE ? tile_at(2 * it) : tile_at(it);
-                if (tile >= total) break;
-                const int as = it & 1;
-                const uint32_t aphase = (it >> 1) & 1;
-                uint32_t tacc = tmem_base + as * 256, tacc1 = 0;
-                if (WIDE) {       // virtual tiles 2*it, 2*it+1 -> regions v % 3, each on its (v / 3)-th use
-                    const int v0 = 2 * it, v1 = 2 * it + 1;
-                    mbar_wait(&tempty[v0 % 3], ((v0 / 3) & 1) ^ 1);
-                    mbar_wait(&tempty[v1 % 3], ((v1 / 3) & 1) ^ 1);
-                    tacc = tmem_base + (v0 % 3) * BN;
-                    tacc1 = tmem_base + (v1 % 3) * BN;
-                } else {
-                    mbar_wait(&tempty[as], aphase ^ 1);
-                }
-                tc_fence_after();
-                const int ntile = WIDE ? BN : min(BN, ((p.N - (tile % p.n_tiles) * BN) + 15) & ~15);
-                const uint32_t idesc = make_idesc_f16(PAIR ? 256 : 128, (uint32_t)ntile, 0, 0);
-                for (int q0 = 0; q0 < kiters; q0 += KC) {
-                    const int nch = min(KC, kiters - q0);
-                    mbar_wait(&full[stage], phase);
-                    tc_fence_after();
-#pragma unroll
-                    for (int c = 0; c < KC; c++) {
-                        if (c < nch) {
-                            const uint64_t ad = make_desc_sw128(smem_u32(sA + (stage * KC + c) * TC_A_BYTES), 16, 1024);
-                            const uint64_t bd = make_desc_sw128(smem_u32(sB + (stage * KC + c) * B_BYTES), 16, 1024);
-#pragma unroll
-                            for (int k = 0; k < 4; k++) { // 4 x (K=16) inside the 64-wide swizzle atom: +32 B each
-                                const uint32_t acc = (q0 + c + k) != 0;
-                                if (PAIR) umma_f16_ss_2cta(tacc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, acc);
-                                else umma_f16_ss(tacc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, acc);
-                                if (WIDE)     // second N-half: same A tile, its weight rows B_BYTES/2 further (>> 4 in the descriptor)
-                                    umma_f16_ss_2cta(tacc1, ad + (uint64_t)(k * 2), bd + (uint64_t)(B_BYTES / 32 + k * 2), idesc, acc);
-                            }
-                        }
-                    }
-                    if (PAIR) umma_commit_2cta_mc(&empty[stage], (uint16_t)0x3);
-                    else if (CL == 2) umma_commit_mc(&empty[stage], (uint16_t)0x3);
-                    else umma_commit(&empty[stage]);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-                if (PAIR) umma_commit_2cta_mc(&tfull[as], (uint16_t)0x3); else umma_commit(&tfull[as]);
-            }
-        }
+        return;
     }
-    } else {
-        if (NWG == 3) asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
-        // ===================== epilogue: NWG warpgroups, spans dealt round-robin across the CTA's tile stream =====================
-        const int g = (warp - 4) >> 2;              // epilogue warpgroup (own staging buffers, own named barrier)
-        const int q = warp & 3;                     // TMEM lane quadrant of this warp
-        const int r = q * 32 + lane;                // tile row of this thread (= TMEM lane)
-        const bool leader = ((threadIdx.x & 127) == 0);   // issues this warpgroup's TMA loads / stores
-        const bool has_res = p.has_r1 || p.has_r2;
-        const uint32_t rbytes = (p.has_r1 ? (p.r1f32 ? 16384u : 8192u) : 0u) + (p.has_r2 ? (p.r2f32 ? 16384u : 8192u) : 0u);
-        uint8_t* myObase = sO + g * p.obufs * OT;
-        uint8_t* myR1 = sR1 + g * p.rbufs * RT1;
-        uint8_t* myR2 = sR2 + g * p.rbufs * RT2;
-        uint32_t pfc = 0;                           // residual chunks prefetched by this warpgroup's leader
-        float* myBias = sBias + g * 256;
-        const int bar_id = 1 + g;
-        constexpr int BAR_ALL = NWG + 1;            // named barrier of all epilogue threads (statistics flush)
-        // One span = one staging tile = one TMA store with 128-byte rows whenever possible (32 fp32 / 64 fp16 / 64 GEGLU output
-        // columns). Narrow-row stores made the TMA store engine the bottleneck of the K=320 GEMMs (profiles/r1_notes.md §1, v6).
-        const int span = p.of32 ? 32 : (p.geglu ? 128 : 64);
-        auto nspans = [&](int tile) { return (min(BN, p.N - (tile % p.n_tiles) * BN) + span - 1) / span; };
-
-        // residual prefetcher (leader only): walks this warpgroup's (tile, span, chunk) sequence one chunk ahead.
-        // pf_G = spans of the CTA's earlier tiles mod NWG; span pf_s of pf_tile is mine iff (pf_G + pf_s) % NWG == g.
-        int pf_i = 0, pf_tile = tile_at(0), pf_G = 0, pf_s = g, pf_cc = 0;
-        auto prefetch_residual = [&]() {
-            while (pf_tile < total) {                                  // skip tiles where this warpgroup has no span (left)
-                const int ns = nspans(pf_tile);
-                if (pf_s < ns) break;
-                pf_G = (pf_G + ns) % NWG; pf_tile = tile_at(++pf_i); pf_s = (g + NWG - pf_G) % NWG; pf_cc = 0;
-            }
-            if (pf_tile >= total) return;
-            const int nt = pf_tile % p.n_tiles, mt = (pf_tile / p.n_tiles) * CL + crank;
-            const int tx = mt % p.ntx, ty = (mt / p.ntx) % p.nty, tz = mt / (p.ntx * p.nty);
-            const int s0 = pf_s * span;
-            const int ncol = nt * BN + s0 + pf_cc;
-            const uint32_t pb = p.rbufs == 2 ? (pfc & 1) : 0;
-            pfc++;
-            mbar_expect_tx(&rfull[2 * g + pb], rbytes);
-            if (p.has_r1) tma_load_4d(&mapR1, myR1 + pb * RT1, &rfull[2 * g + pb], ncol, tx * TW, ty * TH, tz * TN);
-            if (p.has_r2) tma_load_4d(&mapR2, myR2 + pb * RT2, &rfull[2 * g + pb], ncol, tx * TW, ty * TH, tz * TN);
-            const int width = min(span, min(BN - s0, p.N - nt * BN - s0));
-            pf_cc += 32;
-            if (pf_cc >= width) { pf_cc = 0; pf_s += NWG; }
-        };
-        // with rbufs == 2 two residual chunks are always in flight per warpgroup: with one, each SM had at most 32 KB of loads
-        // outstanding (148 SMs x 32 KB / ~1.5 us HBM latency ~ 3.2 TB/s) — the measured ceiling of the fp32-residual linears
-        if (leader && has_res) { prefetch_residual(); if (p.rbufs == 2) prefetch_residual(); }
-
-        uint32_t ci = 0, rc = 0;                    // spans / residual chunks processed by this warpgroup
-        int it = 0, G = 0;
-        // gn_acc: many consecutive tiles of this CTA lie in the same image (VAE: 14 frames or ONE clip over 64 512 tiles),
-        // where per-tile global fp64 atomics serialise on 64 addresses in L2 (measured: 2.7 -> 5-6 ms per full-resolution
-        // conv). Each epilogue warp then sums into its own shared-memory table (plain adds in a fixed order: deterministic)
-        // and the CTA flushes the tables with fp64 atomics when the image changes.
-        int cur_img = -1;
-        float* myStat = sStat + (warp - 4) * 64;
-        auto flush_stats = [&]() {
-            named_bar_sync(BAR_ALL, 128 * NWG);                    // all warpgroups' adds for cur_img are done
-            if (g == 0 && (threadIdx.x & 127) < 64) {
-                const int i = threadIdx.x & 127;
-                double v = 0.0;
-#pragma unroll
-                for (int w = 0; w < 4 * NWG; w++) { v += (double)sStat[w * 64 + i]; sStat[w * 64 + i] = 0.f; }
-                if (v != 0.0) atomicAdd(p.gn_stats + (int64_t)cur_img * p.gn_groups * 2 + i, v);
-            }
-            named_bar_sync(BAR_ALL, 128 * NWG);
-        };
-        if (p.gn_acc) {
-            myStat[lane] = 0.f; myStat[lane + 32] = 0.f;
-            named_bar_sync(BAR_ALL, 128 * NWG);
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // ===================== consumers =====================
+    const int cw = (warp >> 2) - 1;                 // consumer warpgroup: tile rows [64*cw, 64*cw + 64)
+    const int cwarp = warp - 4;                     // consumer warp 0..7
+    const int ct = threadIdx.x - 128;               // consumer thread 0..255
+    const int rl = cw * 64 + (warp & 3) * 16 + (lane >> 2);    // tile row of acc[4i], acc[4i+1]; rl + 8: acc[4i+2], acc[4i+3]
+    const int cb = 2 * (lane & 3);
+    int stage = 0;
+    uint32_t phase = 0;
+    // GroupNorm statistics: consumer thread g < gn_groups owns group g of the current image and flushes it (fp64 atomics)
+    // when the CTA's tile stream moves to another image — tiles of one image are many, the atomics per image few.
+    int cur_img = -1;
+    double st1 = 0.0, st2 = 0.0;
+    auto flush = [&]() {
+        if (cur_img >= 0 && ct < p.gn_groups && (st1 != 0.0 || st2 != 0.0)) {
+            double* dst = p.gn_stats + ((int64_t)cur_img * p.gn_groups + ct) * 2;
+            atomicAdd(dst, st1);
+            atomicAdd(dst + 1, st2);
         }
-        for (;; it++) {
-            const int tile = tile_at(it);
-            if (tile >= total) break;
-            // WIDE: `it` counts virtual tiles; its pass is it >> 1 (accumulator-full barrier of the pass), its TMEM region it % 3
-            const int as = WIDE ? ((it >> 1) & 1) : (it & 1);
-            const uint32_t aphase = WIDE ? ((it >> 2) & 1) : ((it >> 1) & 1);
-            const int te = WIDE ? it % 3 : as;          // tempty barrier of this accumulator
-            const int nt = tile % p.n_tiles;
-            const int mt = (tile / p.n_tiles) * CL + crank;
-            const int tx = mt % p.ntx;
-            const int ty = (mt / p.ntx) % p.nty;
-            const int tz = mt / (p.ntx * p.nty);
-            const int n0 = nt * BN;
-            const int ns = nspans(tile);
-            const int s_first = (g + NWG - G) % NWG;             // my first span of this tile (>= ns: none)
-            G = (G + ns) % NWG;
-            if (p.gn_acc && mt < m_tiles) {
-                const int64_t row0 = ((int64_t)(tz * TN) * p.Yo + ty * TH) * p.Xo + tx * TW;
-                const int img = (int)(row0 / p.gn_rpi);
-                if (img != cur_img) {
-                    if (cur_img >= 0) flush_stats();
-                    cur_img = img;
+        st1 = st2 = 0.0;
+    };
+
+    float acc[NACC];
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+        const int nt = tile % p.n_tiles;
+        const int mt = tile / p.n_tiles;
+        const int tx = mt % p.ntx;
+        const int ty = (mt / p.ntx) % p.nty;
+        const int tz = mt / (p.ntx * p.nty);
+        const int n0 = nt * BN;
+#pragma unroll
+        for (int i = 0; i < NACC; i++) acc[i] = 0.f;
+        int prev = -1;
+        for (int q = 0; q < kiters; q++) {
+            mbar_wait(&full[stage], phase);
+            const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+            const uint64_t ad = make_desc_sw128(sa + cw * (64 * 128), 16, 1024);
+            const uint64_t bd = make_desc_sw128(sa + TC_A_BYTES, 16, 1024);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; k++) {           // 4 x (K=16) inside the 64-wide swizzle atom: +32 B each
+                if constexpr (BN == 256) wgmma_m64n256_ss(acc, ad + 2 * k, bd + 2 * k, 1u);
+                else if constexpr (BN == 160) wgmma_m64n160_ss(acc, ad + 2 * k, bd + 2 * k, 1u);
+                else wgmma_m64n128_ss(acc, ad + 2 * k, bd + 2 * k, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                        // the previous stage's batch is done: release its buffers
+            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+            prev = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+
+        // ---- epilogue: output rows of this thread (-1: outside the output)
+        int64_t grow[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int r = rl + 8 * h;
+            const int x = tx * TW + (r & (TW - 1));
+            const int y = ty * TH + ((r >> p.lTW) & (TH - 1));
+            const int z = tz * TN + (r >> (p.lTW + p.lTH));
+            grow[h] = (x < p.Xo && y < p.Yo && z < p.Zo) ? ((int64_t)z * p.Yo + y) * p.Xo + x : -1;
+        }
+        if (p.geglu) {
+            // value columns 32b + [0,16), gate columns 32b + [16,32) of the accumulator -> output columns 16b + [0,16)
+            act_t* out = reinterpret_cast<act_t*>(p.out);
+#pragma unroll
+            for (int i = 0; i < BN / 8; i++) {
+                if ((i & 3) >= 2) continue;
+                const int col = n0 + 8 * i + cb;
+                const float2 bv = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
+                const float2 bg = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col + 16)) : make_float2(0.f, 0.f);
+                const int oc = (n0 >> 1) + 16 * (i >> 2) + 8 * (i & 3) + cb;
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    if (grow[h] < 0) continue;
+                    const float o0 = geglu(acc[4 * i + 2 * h] + bv.x, acc[4 * (i + 2) + 2 * h] + bg.x);
+                    const float o1 = geglu(acc[4 * i + 2 * h + 1] + bv.y, acc[4 * (i + 2) + 2 * h + 1] + bg.y);
+                    *reinterpret_cast<uint32_t*>(out + grow[h] * p.ldo + oc) = pack2(o0, o1);
                 }
             }
-            const float* rv = nullptr;
-            if (s_first < ns) {
-                // per-row vector (emb_layers add / len-1 cross-attention bias): when every row of the tile reads the SAME vector
-                // (a tile inside one frame / clip — always, for the UNet's shapes) it is folded into the staged bias slice
-                const float* rv_tile = nullptr;
-                if (p.rowvec) {
-                    const int x0 = tx * TW, y0 = ty * TH, z0 = tz * TN;
-                    if (x0 < p.Xo && y0 < p.Yo && z0 < p.Zo) {
-                        const int x1 = min(x0 + TW, p.Xo) - 1, y1 = min(y0 + TH, p.Yo) - 1, z1 = min(z0 + TN, p.Zo) - 1;
-                        const int64_t i0 = (((int64_t)z0 * p.Yo + y0) * p.Xo + x0) / p.rpv, i1 = (((int64_t)z1 * p.Yo + y1) * p.Xo + x1) / p.rpv;
-                        if (i0 == i1) rv_tile = p.rowvec + i0 * (int64_t)p.ldv;
-                    }
-                    if (!rv_tile) {
-                        const int x = x0 + (r & (TW - 1));
-                        const int y = y0 + ((r >> p.lTW) & (TH - 1));
-                        const int z = z0 + (r >> (p.lTW + p.lTH));
-                        if (x < p.Xo && y < p.Yo && z < p.Zo)
-                            rv = p.rowvec + ((((int64_t)z * p.Yo + y) * p.Xo + x) / p.rpv) * (int64_t)p.ldv;
-                    }
-                }
-                for (int j = threadIdx.x & 127; j < BN; j += 128) {
-                    float b = 0.f;
-                    if (n0 + j < p.N) {
-                        if (p.bias) b = __ldg(p.bias + n0 + j);
-                        if (rv_tile) b += __ldg(rv_tile + n0 + j);
-                    }
-                    myBias[j] = b;
-                }
-                named_bar_sync(bar_id, 128);                  // B0: bias slice staged (the previous tile's reads ended at its last B2)
-            }
-            // also taken without a span in this tile: arriving on tempty below is only legal once the accumulator's previous
-            // phase is over, which tfull of THIS tile implies (the MMA waited for it)
-            mbar_wait(&tfull[as], aphase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (WIDE ? (it % 3) * BN : as * 256);
-#pragma unroll 1
-            for (int si = s_first; si < ns; si += NWG, ci++) {
-                const int s0 = si * span;
-                uint8_t* myO = myObase + (p.obufs == 2 ? (ci & 1) * OT : 0);
-                const int width = min(span, min(BN - s0, p.N - n0 - s0));      // accumulator columns in this span
-                const bool wide = p.of32 || p.geglu || width > 32;             // 128-byte staging rows (SWIZZLE_128B)
-                if (leader) {                                                  // the store that last used myO has drained it
-                    if (p.obufs == 2) bulk_wait_read<1>(); else bulk_wait_read<0>();
-                }
-                named_bar_sync(bar_id, 128);                                   // B1: myO is free
-#pragma unroll 1
-                for (int cc = 0; cc < width; cc += 32) {
-                    const int c0 = s0 + cc;
-                    uint32_t v[32];
-                    tmem_ld32(taddr + c0, v);
-                    tmem_ld_wait();
-                    const int n = n0 + c0;
-                    if (rv) {                                                  // rows of this tile read different vectors (rare)
-                        if (n + 32 <= p.N) {
+            continue;
+        }
+        const float* rv[2] = {nullptr, nullptr};
+        if (p.rowvec) {
 #pragma unroll
-                            for (int j = 0; j < 32; j += 4) {
-                                const float4 t = __ldg(reinterpret_cast<const float4*>(rv + n + j));
-                                v[j] = __float_as_uint(__uint_as_float(v[j]) + t.x); v[j + 1] = __float_as_uint(__uint_as_float(v[j + 1]) + t.y);
-                                v[j + 2] = __float_as_uint(__uint_as_float(v[j + 2]) + t.z); v[j + 3] = __float_as_uint(__uint_as_float(v[j + 3]) + t.w);
-                            }
-                        } else {                                               // ragged N tail
-#pragma unroll 1
-                            for (int j = 0; j < p.N - n; j++) {
-                                const float add = rv[n + j];
+            for (int h = 0; h < 2; h++)
+                if (grow[h] >= 0) rv[h] = p.rowvec + (grow[h] / p.rpv) * (int64_t)p.ldv;
+        }
+        const bool stats = p.gn_stats != nullptr;
 #pragma unroll
-                                for (int k = 0; k < 32; k++) if (k == j) v[k] = __float_as_uint(__uint_as_float(v[k]) + add);
-                            }
-                        }
+        for (int i = 0; i < BN / 8; i++) {
+            const int col = n0 + 8 * i + cb;
+            const bool c0ok = col < p.N, c1ok = col + 1 < p.N;
+            float s1a = 0.f, s2a = 0.f, s1b = 0.f, s2b = 0.f;   // statistics of columns col, col + 1 over this thread's rows
+            if (c0ok) {
+                float2 b = make_float2(0.f, 0.f);
+                if (p.bias) b = c1ok ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(__ldg(p.bias + col), 0.f);
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    if (grow[h] < 0) continue;
+                    float v0 = acc[4 * i + 2 * h] + b.x, v1 = acc[4 * i + 2 * h + 1] + b.y;
+                    if (rv[h]) { v0 += rv[h][col]; if (c1ok) v1 += rv[h][col + 1]; }
+                    if (p.act == 1) { v0 = silu(v0); v1 = silu(v1); }
+                    v0 *= p.a0; v1 *= p.a0;
+                    if (p.res1) {
+                        const int64_t o = grow[h] * p.ld1 + col;
+                        if (c1ok) { const float2 t = ld_res2(p.res1, p.r1f32, o); v0 += p.a1 * t.x; v1 += p.a1 * t.y; }
+                        else v0 += p.a1 * ld_res(p.res1, p.r1f32, o);
                     }
-                    uint64_t x2[16];                                           // accumulator + bias, packed fp32 pairs (FADD2)
-#pragma unroll
-                    for (int j = 0; j < 16; j += 2) {                          // bias slice from smem (warp-broadcast reads)
-                        const float4 t = *reinterpret_cast<const float4*>(myBias + c0 + 2 * j);
-                        x2[j] = add2f(pk2f(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1])), pk2f(t.x, t.y));
-                        x2[j + 1] = add2f(pk2f(__uint_as_float(v[2 * j + 2]), __uint_as_float(v[2 * j + 3])), pk2f(t.z, t.w));
+                    if (p.res2) {
+                        const int64_t o = grow[h] * p.ld2 + col;
+                        if (c1ok) { const float2 t = ld_res2(p.res2, p.r2f32, o); v0 += p.a2 * t.x; v1 += p.a2 * t.y; }
+                        else v0 += p.a2 * ld_res(p.res2, p.r2f32, o);
                     }
-                    if (p.geglu) {                             // value columns 0..15, gate columns 16..31 -> 16 outputs of a 128-byte row
-                        uint32_t pw[8];
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            float o0, o1;
-                            upk2f(geglu_pair(x2[j], x2[8 + j]), o0, o1);
-                            pw[j] = pack2(o0, o1);
-                        }
-#pragma unroll
-                        for (int c = 0; c < 2; c++)
-                            *reinterpret_cast<uint4*>(myO + stg_off(r, (cc >> 5) * 2 + c, 8, 0)) =
-                                make_uint4(pw[4 * c], pw[4 * c + 1], pw[4 * c + 2], pw[4 * c + 3]);
-                        continue;
-                    }
-                    float xf[32];
-#pragma unroll
-                    for (int j = 0; j < 16; j++) upk2f(x2[j], xf[2 * j], xf[2 * j + 1]);
-                    if (p.act == 1) {
-#pragma unroll
-                        for (int j = 0; j < 32; j++) xf[j] = silu(xf[j]);
-                    }
-                    if (p.a0 != 1.0f) {
-#pragma unroll
-                        for (int j = 0; j < 32; j++) xf[j] *= p.a0;
-                    }
-                    if (has_res) {
-                        const uint32_t rb = p.rbufs == 2 ? (rc & 1) : 0;
-                        mbar_wait(&rfull[2 * g + rb], (p.rbufs == 2 ? (rc >> 1) : rc) & 1);
-                        rc++;
-                        if (p.has_r1) add_residual_row(xf, myR1 + rb * RT1, r, p.r1f32, p.a1);
-                        if (p.has_r2) add_residual_row(xf, myR2 + rb * RT2, r, p.r2f32, p.a2);
-                        if (cc + 32 < width) {                                 // more chunks in this span: recycle the buffer now
-                            named_bar_sync(bar_id, 128);
-                            if (leader) prefetch_residual();
-                        }
-                    }
+                    const int64_t o = grow[h] * p.ldo + col;
                     if (p.of32) {
-#pragma unroll
-                        for (int c = 0; c < 8; c++)
-                            *reinterpret_cast<uint4*>(myO + stg_off(r, c, 8, 0)) =
-                                make_uint4(__float_as_uint(xf[4 * c]), __float_as_uint(xf[4 * c + 1]),
-                                           __float_as_uint(xf[4 * c + 2]), __float_as_uint(xf[4 * c + 3]));
-                    } else {                                   // 32 output columns: half of a 128-byte row, or a 64-byte row
-#pragma unroll
-                        for (int c = 0; c < 4; c++)
-                            *reinterpret_cast<uint4*>(myO + (wide ? stg_off(r, (cc >> 5) * 4 + c, 8, 0) : stg_off(r, c, 4, 1))) =
-                                make_uint4(pack2(xf[8 * c], xf[8 * c + 1]), pack2(xf[8 * c + 2], xf[8 * c + 3]),
-                                           pack2(xf[8 * c + 4], xf[8 * c + 5]), pack2(xf[8 * c + 6], xf[8 * c + 7]));
+                        float* out = reinterpret_cast<float*>(p.out);
+                        if (c1ok) *reinterpret_cast<float2*>(out + o) = make_float2(v0, v1);
+                        else out[o] = v0;
+                    } else {
+                        act_t* out = reinterpret_cast<act_t*>(p.out);
+                        const uint32_t w = pack2(v0, v1);
+                        if (c1ok) *reinterpret_cast<uint32_t*>(out + o) = w;
+                        else out[o] = f2act(v0);
+                        const float2 r = unpack2(w);             // statistics of the stored (rounded) values
+                        v0 = r.x; v1 = r.y;
                     }
-                }
-                fence_proxy_async_smem();
-                named_bar_sync(bar_id, 128);                  // B2: span staged; residual buffer fully consumed
-                if (leader) {
-                    const int ncol = p.geglu ? ((n0 + s0) >> 1) : (n0 + s0);
-                    tma_store_4d(wide ? &mapO : &mapO2, myO, ncol, tx * TW, ty * TH, tz * TN);
-                    bulk_commit();
-                    if (has_res) prefetch_residual();         // first chunk of this warpgroup's next span
-                }
-                if (p.gn_stats && mt < m_tiles) {
-                    // Fused GroupNorm statistics: lane = column of a 32-column chunk; each warp sums its own 32 staged
-                    // rows (exactly the stored values), then a segmented warp scan folds the columns of each group.
-#pragma unroll 1
-                    for (int cc = 0; cc < width; cc += 32) {
-                        const int col = n0 + s0 + cc + lane;
-                        float s1 = 0.f, s2 = 0.f;
-                        if (col < p.N) {
-                            // (fully unrolling this loop with independent accumulators measured 1.6x SLOWER: the epilogue's
-                            // instruction footprint is what the 32 KB instruction cache tolerates, see profiles/r1_notes.md §1)
-#pragma unroll 4
-                            for (int rr = 0; rr < 32; rr++) {
-                                const int row = q * 32 + rr;
-                                float val;
-                                if (p.of32) val = *reinterpret_cast<const float*>(myO + stg_off(row, lane >> 2, 8, 0) + (lane & 3) * 4);
-                                else if (wide) val = act2f(*reinterpret_cast<const act_t*>(myO + stg_off(row, (cc + lane) >> 3, 8, 0) + (lane & 7) * 2));
-                                else val = act2f(*reinterpret_cast<const act_t*>(myO + stg_off(row, lane >> 3, 4, 1) + (lane & 7) * 2));
-                                s1 += val; s2 += val * val;
-                            }
-                        }
-                        const int gl = col % p.gn_cpg;        // position inside the channel group
-#pragma unroll
-                        for (int off = 1; off < 32; off <<= 1) {
-                            const float t1 = __shfl_up_sync(0xffffffffu, s1, off), t2 = __shfl_up_sync(0xffffffffu, s2, off);
-                            if (gl >= off && lane >= off) { s1 += t1; s2 += t2; }
-                        }
-                        const bool last = (gl == p.gn_cpg - 1) || lane == 31 || col == p.N - 1;
-                        if (last && col < p.N) {
-                            if (p.gn_acc) {
-                                myStat[(col / p.gn_cpg) * 2] += s1;        // one lane per group: no conflicts inside the warp
-                                myStat[(col / p.gn_cpg) * 2 + 1] += s2;
-                            } else {
-                                const int64_t row0 = ((int64_t)(tz * TN) * p.Yo + ty * TH) * p.Xo + tx * TW;
-                                double* dst = p.gn_stats + ((row0 / p.gn_rpi) * p.gn_groups + col / p.gn_cpg) * 2;
-                                atomicAdd(dst, (double)s1);
-                                atomicAdd(dst + 1, (double)s2);
-                            }
-                        }
-                    }
+                    s1a += v0; s2a += v0 * v0;
+                    if (c1ok) { s1b += v1; s2b += v1 * v1; }
                 }
             }
-            tc_fence_before();
-            if (PAIR) mbar_arrive_cluster(&tempty[te], 0); else mbar_arrive(&tempty[te]);
+            if (stats) {                            // fold the 8 row-groups of the warp (lanes with equal lane % 4)
+#pragma unroll
+                for (int off = 4; off < 32; off <<= 1) {
+                    s1a += __shfl_xor_sync(0xffffffffu, s1a, off); s2a += __shfl_xor_sync(0xffffffffu, s2a, off);
+                    s1b += __shfl_xor_sync(0xffffffffu, s1b, off); s2b += __shfl_xor_sync(0xffffffffu, s2b, off);
+                }
+                if (lane < 4) {
+                    float* d = sStat + (cwarp * BN + 8 * i + cb) * 2;
+                    d[0] = s1a; d[1] = s2a; d[2] = s1b; d[3] = s2b;
+                }
+            }
         }
-        if (p.gn_acc && cur_img >= 0) flush_stats();
-        if (leader) bulk_wait_read<0>();
+        if (stats) {
+            // fixed summation order (warps, then columns of the group): the statistics do not depend on scheduling
+            named_bar_sync(1, 256);
+            if (ct < BN) {
+                float a = 0.f, b = 0.f;
+#pragma unroll
+                for (int w = 0; w < 8; w++) { a += sStat[(w * BN + ct) * 2]; b += sStat[(w * BN + ct) * 2 + 1]; }
+                sStat[ct * 2] = a; sStat[ct * 2 + 1] = b;
+            }
+            named_bar_sync(1, 256);
+            const int64_t row0 = ((int64_t)(tz * TN) * p.Yo + ty * TH) * p.Xo + tx * TW;
+            const int img = (int)(row0 / p.gn_rpi);
+            if (img != cur_img) { flush(); cur_img = img; }
+            if (ct < p.gn_groups) {
+                const int lo = max(ct * p.gn_cpg, n0), hi = min(min((ct + 1) * p.gn_cpg, n0 + BN), p.N);
+                for (int c = lo; c < hi; c++) { st1 += (double)sStat[(c - n0) * 2]; st2 += (double)sStat[(c - n0) * 2 + 1]; }
+            }
+            named_bar_sync(1, 256);                 // sStat is rewritten by the next tile
+        }
     }
-
-    tc_fence_before();
-    if (CL == 2) cluster_sync_all(); else __syncthreads();     // no CTA leaves while its peer can still signal / write into it
-    if (warp == 2) {
-        tc_fence_after();
-        if (PAIR) tmem_dealloc_2cta(tmem_base, 512); else tmem_dealloc(tmem_base, 512);
-    }
+    if (p.gn_stats) flush();
 }
 
 // ------------------------------------------------------------------------------------------------ host launcher
@@ -635,94 +361,46 @@ static int ilog2(int v) {
     return l;
 }
 
-constexpr int TC_RETRY_NWG2 = 77;
-template <int BN, int MODE, int NWG, int KC = ((BN <= 160 && MODE == 3) ? 2 : 1)>   // (mode 4: KC = 1)
-static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mO, const CUtensorMap& mO2,
-                     const CUtensorMap& mR1, const CUtensorMap& mR2, TcParams& p, cudaStream_t st) {
+static int num_sms_cached() {
+    static const int n = [] { int d = 0, v = 0; cudaGetDevice(&d); cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, d); return v; }();
+    return n;
+}
+
+template <int BN>
+static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, TcParams& p, cudaStream_t st) {
     static bool configured = false;
-    static int num_sms = 0;
-    constexpr int CL = MODE >= 2 ? 2 : 1;
-    // measured in one run (tools/bench_convgemm.py, conv 320->320 @ 28x72x128, pair mode): KC=1 1000, KC=2 1126 TFLOP/s;
-    // in mode 2 the doubled stage leaves only 2 stages for BN=160 and is slower.
-    constexpr int STAGE_BYTES = KC * (TC_A_BYTES + (MODE == 4 ? BN * 128 : MODE == 3 ? BN * 64 : BN * 128));
     if (!configured) {
-        GCD_CUDA_CHECK(cudaFuncSetAttribute(tc_gemm_kernel<BN, MODE, KC, NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
-        int dev = 0;
-        GCD_CUDA_CHECK(cudaGetDevice(&dev));
-        GCD_CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
+        GCD_CUDA_CHECK(cudaFuncSetAttribute(tc_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
         configured = true;
     }
-    const int OT = 16384;
-    const int RT = (p.has_r1 ? (p.r1f32 ? 16384 : 8192) : 0) + (p.has_r2 ? (p.r2f32 ? 16384 : 8192) : 0);
-    const int kiters = p.ntaps * p.kchunks;
-    // short K loop => the epilogue is the critical path: double-buffer its staging tiles if >= 3 pipeline stages remain
-    // very short K loops (K <= 384) with a residual are bound by the epilogue's HBM round trips, not by operand delivery: two
-    // pipeline stages suffice there and the shared memory goes to double-buffered residual AND output staging tiles
-    static const int minst_env = [] { const char* e = getenv("GCD_TC_MINST"); return e ? atoi(e) : 2; }();
-    const int need = (kiters <= 6 && RT > 0) ? minst_env : 3;
-    auto plan = [&](int fixed, int& obufs, int& stages) {
-        // short K loop: first keep two residual chunks in flight (HBM latency), then double-buffer the output staging
-        p.rbufs = (RT > 0 && kiters <= 24 && (TC_SMEM_MAX - (NWG * OT + 2 * NWG * RT) - fixed - 256) / STAGE_BYTES >= need) ? 2 : 1;
-        obufs = (kiters <= 24 && (TC_SMEM_MAX - (2 * NWG * OT + NWG * p.rbufs * RT) - fixed - 256) / STAGE_BYTES >= need) ? 2 : 1;
-        stages = (TC_SMEM_MAX - (NWG * obufs * OT + NWG * p.rbufs * RT + fixed) - 256) / STAGE_BYTES;
-        if (stages > 8) stages = 8;
-    };
-    p.gn_acc = 0;
-    int fixed = NWG * 1024 /*bias slices*/, stages;
-    plan(fixed, p.obufs, stages);
-    if (p.gn_stats) {
-        // consecutive tiles of a CTA are num_sms M-tiles apart: accumulate per CTA when an image spans many such strides ...
-        const int64_t rows = (int64_t)p.Xo * p.Yo * p.Zo;
-        const int64_t n_img = (rows + p.gn_rpi - 1) / p.gn_rpi;
-        int ob2, st2;
-        plan(fixed + NWG * 1024, ob2, st2);
-        // ... unless the 2 KB of tables would leave fewer than 4 pipeline stages (then keep the direct global atomics)
-        if (p.gn_groups == 32 && (int64_t)p.ntx * p.nty * p.ntz / n_img >= 4 * (int64_t)num_sms && ob2 == p.obufs && (st2 == stages || st2 >= 4)) {
-            p.gn_acc = 1;
-            fixed += NWG * 1024;
-        }
-        plan(fixed, p.obufs, stages);          // final plan (also restores rbufs when the tables were rejected)
-    }
-    const int epi = NWG * p.obufs * OT + NWG * p.rbufs * RT + fixed;
-    if (NWG == 3 && stages < 3) return TC_RETRY_NWG2;      // the third warpgroup's staging tiles would starve the operand pipeline
+    constexpr int STAGE_BYTES = TC_A_BYTES + BN * 128;
+    const int fixed = (p.gn_stats ? 8 * BN * 2 * 4 : 0) + 256;     // statistics table + barriers
+    int stages = (TC_SMEM_MAX - fixed) / STAGE_BYTES;
+    if (stages > 8) stages = 8;
     GCD_REQUIRE(stages >= 2, "tc_gemm: not enough shared memory for the pipeline (BN=%d)", BN);
     p.stages = stages;
-    const int smem = stages * STAGE_BYTES + epi + 256;
-    const int m_tiles = p.ntx * p.nty * p.ntz;
-    const int groups = ((m_tiles + CL - 1) / CL) * p.n_tiles;
-    const int max_clusters = num_sms / CL;
-    const int grid = (groups < max_clusters ? groups : max_clusters) * CL;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(128 + 128 * NWG);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    GCD_CUDA_CHECK(cudaLaunchKernelEx(&cfg, tc_gemm_kernel<BN, MODE, KC, NWG>, mA, mB, mO, mO2, mR1, mR2, p));
+    const int smem = stages * STAGE_BYTES + fixed;
+    const int tiles = p.ntx * p.nty * p.ntz * p.n_tiles;
+    const int sms = num_sms_cached();
+    GCD_REQUIRE(sms > 0, "tc_gemm: no CUDA device");
+    const int grid = tiles < sms ? tiles : sms;
+    tc_gemm_kernel<BN><<<grid, TC_THREADS, smem, st>>>(mA, mB, p);
+    GCD_CUDA_CHECK(cudaGetLastError());
     g_launches++;
     return 0;
 }
 
-// 4-D map over an output-shaped tensor [Z, Y, X, cols] with leading dimension ld (elements), box = tile x `bcols`.
-static int make_out_map(CUtensorMap* m, const void* ptr, int f32, int ld, int cols, int Xo, int Yo, int Zo, int TW, int TH,
-                        int TN, int bcols, const char* what) {
+// 16-byte alignment of an epilogue tensor and its rows (vector loads / stores of column pairs)
+static int check_ep_tensor(const void* ptr, int f32, int ld, const char* what) {
     const int es = f32 ? 4 : 2;
     GCD_REQUIRE(((uintptr_t)ptr & 15) == 0 && ((int64_t)ld * es) % 16 == 0,
                 "gcd_tc_run: %s must be 16-byte aligned with a leading dimension multiple of 16 bytes (ld=%d)", what, ld);
-    uint64_t dims[4] = {(uint64_t)cols, (uint64_t)Xo, (uint64_t)Yo, (uint64_t)Zo};
-    uint64_t str[3] = {(uint64_t)ld * es, (uint64_t)ld * es * Xo, (uint64_t)ld * es * Xo * Yo};
-    uint32_t box[4] = {(uint32_t)bcols, (uint32_t)TW, (uint32_t)TH, (uint32_t)TN};
-    return gcd_make_tmap(m, ptr, 4, dims, str, box, nullptr, bcols * es, f32);
+    return 0;
 }
 
 // ---- tensor-map cache (host)
-struct TmapKey { gcd_tc_op op; int bn, cl; };
-struct TmapSet { CUtensorMap m[6]; };
+struct TmapKey { gcd_tc_op op; int bn; };
+struct TmapSet { CUtensorMap m[2]; };
 struct TmapKeyHash {
     size_t operator()(const TmapKey& k) const {
         const unsigned char* b = reinterpret_cast<const unsigned char*>(&k);
@@ -747,13 +425,9 @@ static void tmap_cache_put(const TmapKey& k, const TmapSet& v) {
     g_tmap_cache.emplace(k, v);
 }
 
-static int nwg_cfg() {
-    static const int v = [] { const char* e = getenv("GCD_TC_NWG"); return (e && atoi(e) == 3) ? 3 : 2; }();
-    return v;
-}
-// Experiments only (tools/autotune_tc.py): force the tile width / cluster mode of the following gcd_tc_run calls (0 = automatic).
-static int g_ovr_bn = 0, g_ovr_mode = 0;
-extern "C" void gcd_tc_override(int bn, int mode) { g_ovr_bn = bn; g_ovr_mode = mode; }
+// Experiments only (tools/autotune_tc.py): force the tile width of the following gcd_tc_run calls (0 = automatic; `mode` is ignored).
+static int g_ovr_bn = 0;
+extern "C" void gcd_tc_override(int bn, int mode) { g_ovr_bn = bn; (void)mode; }
 
 extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
@@ -805,51 +479,30 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
     p.w_batched = op->w_batch_stride != 0;
     GCD_REQUIRE(!p.w_batched || TH == 1, "gcd_tc_run: batched weights need gemm tiling");
 
-    // Tile width: wide MMAs are markedly more efficient (measured per useful column, pair mode: BN=128 ~0.98, 160 ~1.14-1.26,
-    // 256 ~1.43 PFLOP/s; tools/bench_convgemm.py), and the last tile of a row is issued at its real width, so prefer 256
-    // unless that leaves a sliver; N = 320 (2 x 160) is the one shape where 160 wins.
+    // Tile width: the widest wgmma (N = 256) reads each activation tile once per 256 output columns; N = 320 / 640 / 1280
+    // convs split evenly into 160-column tiles. On small problems (the 9x16 / 18x32 levels: M = 4032 rows) wave quantisation
+    // over the SMs decides instead: cost = waves x tile width.
     int BN;
     if (op->N % 256 == 0 || op->N >= 384) BN = 256;
     else if (op->N % 160 == 0) BN = 160;
     else BN = 128;
-    // Small problems (the 9x16 / 18x32 levels: M = 4032 rows -> 16 CTA pairs) are decided by wave quantisation, not by the MMA
-    // width: N = 1280 gives 80 BN=256 pair-tiles on 74 pairs = two waves at 54 % (measured 0.76-0.80 PFLOP/s), 128 BN=160 tiles
-    // = two waves at 86 %. Cost = waves x tile time, tile time ~ BN / measured per-column efficiency of that width.
-    static const int num_sms_h = [] { int d = 0, n = 148; cudaGetDevice(&d); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d); return n; }();
-    if (BN == 256 && !e.geglu && op->w_batch_stride == 0) {
-        const long m_pairs = ((long)p.ntx * p.nty * p.ntz + 1) / 2, slots = num_sms_h / 2;
-        auto cost = [&](int bn, double eff) {
-            const long tiles = m_pairs * ((op->N + bn - 1) / bn);
-            return (double)((tiles + slots - 1) / slots) * bn / eff;
-        };
-        const double c256 = cost(256, 1.43), c160 = cost(160, 1.20);
-        if (m_pairs * ((op->N + 255) / 256) <= 3 * slots && op->N % 160 == 0 && c160 < 0.9 * c256) BN = 160;
+    const int num_sms_h = num_sms_cached();
+    GCD_REQUIRE(num_sms_h > 0, "gcd_tc_run: no CUDA device");
+    if (BN == 256 && !e.geglu && op->N % 160 == 0) {
+        const long m_tiles = (long)p.ntx * p.nty * p.ntz;
+        auto cost = [&](int bn) { return (double)((m_tiles * ((op->N + bn - 1) / bn) + num_sms_h - 1) / num_sms_h) * bn; };
+        if (cost(160) < 0.9 * cost(256)) BN = 160;
     }
-    static const int bn_env = [] { const char* e = getenv("GCD_TC_BN"); return e ? atoi(e) : 0; }();   // experiments only
-    if (bn_env == 128 || bn_env == 160 || bn_env == 256) { if (!e.geglu) BN = bn_env; }
     if ((g_ovr_bn == 128 || g_ovr_bn == 160 || g_ovr_bn == 256) && !e.geglu) BN = g_ovr_bn;
     p.n_tiles = (op->N + BN - 1) / BN;
-    // MODE 3 (CTA pair, cta_group::2 MMA) unless overridden (GCD_TC_MODE=1|2|3), batched weights, or a single M-tile
-    static const int mode_env = [] { const char* e = getenv("GCD_TC_MODE"); return e ? atoi(e) : 3; }();
-    // short K loops are epilogue-bound: the looser coupling of mode 2 (multicast only) measured faster there
-    // K = 320 (5 chunks): mode 2 is 23-30 % faster; K = 640 (10 chunks): the pair MMA is 7-8 % faster with the round-2 epilogue
-    // (tools/bench_ops.py, GCD_TC_AUTO_K=4 vs 10, same box: GEGLU K=640 0.347 vs 0.378 ms, N=640 residual 0.115 vs 0.123)
-    static const int auto_k = [] { const char* e = getenv("GCD_TC_AUTO_K"); return e ? atoi(e) : 9; }();
-    const int auto_mode = (p.ntaps * p.kchunks <= auto_k) ? 2 : 3;
-    int MODE = (mode_env >= 2 && !p.w_batched && p.ntx * p.nty * p.ntz >= 2) ? (mode_env >= 3 ? auto_mode : 2) : 1;
-    if (MODE >= 2 && (g_ovr_mode == 2 || g_ovr_mode == 3)) MODE = g_ovr_mode;
-    // wide tiles (mode 4): N = 320 exactly, pair mode, two warpgroups, and K >= 3840 — measured in situ (tools/prof_forward.py,
-    // same box, GCD_TC_WIDE=0 / GCD_TC_WIDE_K): K=8640 2.43 -> 1.98 ms, K=5760 3.29 -> 3.09, K=2880 4.46 -> 4.52, K <= 1280 slower
-    // (the half-tile epilogue that cannot overlap the next pass is no longer amortised)
-    static const int wide_env = [] { const char* e = getenv("GCD_TC_WIDE"); return e ? atoi(e) : 1; }();
-    static const int wide_k = [] { const char* e = getenv("GCD_TC_WIDE_K"); return e ? atoi(e) : 60; }();
-    if (MODE == 3 && BN == 160 && op->N == 320 && wide_env && nwg_cfg() == 2 && p.ntaps * p.kchunks >= wide_k) MODE = 4;
-    const int CL = MODE >= 2 ? 2 : 1;
 
     p.bias = e.bias; p.rowvec = e.rowvec; p.rpv = e.rows_per_vec; p.ldv = e.ld_rowvec;
-    p.has_r1 = e.res1 != nullptr; p.has_r2 = e.res2 != nullptr; p.r1f32 = e.res1_f32; p.r2f32 = e.res2_f32;
+    p.res1 = e.res1; p.res2 = e.res2; p.ld1 = e.ld_res1; p.ld2 = e.ld_res2; p.r1f32 = e.res1_f32; p.r2f32 = e.res2_f32;
     p.a0 = e.a_acc; p.a1 = e.a_res1; p.a2 = e.a_res2;
-    p.of32 = e.out_f32; p.geglu = e.geglu; p.act = e.act;
+    p.out = e.out; p.ldo = e.ld_out; p.of32 = e.out_f32; p.geglu = e.geglu; p.act = e.act;
+    if (check_ep_tensor(e.out, e.out_f32, e.ld_out, "out")) return -2;
+    if (e.res1 && check_ep_tensor(e.res1, e.res1_f32, e.ld_res1, "res1")) return -2;
+    if (e.res2 && check_ep_tensor(e.res2, e.res2_f32, e.ld_res2, "res2")) return -2;
     int stats_skipped = 0;
     if (e.gn_stats) {
         GCD_REQUIRE(e.gn_cpg > 0 && e.gn_groups > 0 && e.gn_rows_per_img > 0 && !e.geglu, "gcd_tc_run: bad gn_stats arguments");
@@ -860,19 +513,19 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
         else stats_skipped = 1;
     }
 
-    // ---- tensor maps: six cuTensorMapEncodeTiled calls per op, cached per (descriptor, tile width, cluster size) — every forward
+    // ---- tensor maps: two cuTensorMapEncodeTiled calls per op, cached per (descriptor, tile width) — every forward
     // of the eager paths (VAE decode, generic sampler path, the capture pass of the CUDA graph) re-issues the same few hundred ops
-    // on the same pool buffers. The key is the whole gcd_tc_op (pointers, extents, strides, epilogue tensors) + BN + CL.
-    CUtensorMap mA, mB, mO, mO2, mR1, mR2;
+    // on the same pool buffers. The key is the whole gcd_tc_op (pointers, extents, strides, epilogue tensors) + BN.
+    CUtensorMap mA, mB;
     TmapKey tkey;
     memset(&tkey, 0, sizeof(tkey));
-    tkey.op = *op; tkey.bn = BN; tkey.cl = CL;
+    tkey.op = *op; tkey.bn = BN;
     tkey.op.ep.a_acc = tkey.op.ep.a_res1 = tkey.op.ep.a_res2 = 0.f;           // scalars / non-tensor fields do not shape the maps
     tkey.op.ep.bias = nullptr; tkey.op.ep.rowvec = nullptr; tkey.op.ep.gn_stats = nullptr;
     tkey.op.ep.rows_per_vec = tkey.op.ep.ld_rowvec = 0; tkey.op.ep.act = 0; tkey.op.ep.gn_cpg = tkey.op.ep.gn_groups = 0; tkey.op.ep.gn_rows_per_img = 0;
     TmapSet hit;
     if (tmap_cache_find(tkey, &hit)) {
-        mA = hit.m[0]; mB = hit.m[1]; mO = hit.m[2]; mO2 = hit.m[3]; mR1 = hit.m[4]; mR2 = hit.m[5];
+        mA = hit.m[0]; mB = hit.m[1];
     } else {
     {
         uint64_t dims[4] = {(uint64_t)op->C, (uint64_t)op->Xi, (uint64_t)op->Yi, (uint64_t)op->Zi};
@@ -892,56 +545,19 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
         GCD_REQUIRE(op->C % 64 == 0 || op->ntaps == 1, "gcd_tc_run: multi-tap ops need C %% 64 == 0 (got %d)", op->C);
         uint64_t dims[3] = {(uint64_t)op->ntaps * (uint64_t)op->C, (uint64_t)op->N, nb};
         uint64_t str[2] = {(uint64_t)op->ldw * 2, (uint64_t)(p.w_batched ? op->w_batch_stride : op->ldw * (int64_t)op->N) * 2};
-        uint32_t box[3] = {64, (uint32_t)(BN / CL), 1};     // CL == 2: each CTA fetches half of the weight tile
+        uint32_t box[3] = {64, (uint32_t)BN, 1};
         int rc = gcd_make_tmap(&mB, op->W, 3, dims, str, box, nullptr, 128, 0);
         if (rc) return rc;
     }
-    {
-        const int Nout = e.geglu ? op->N / 2 : op->N;
-        // full-width staging tile: 128-byte rows = 32 fp32 / 64 fp16 (incl. GEGLU) columns; mO2: ragged 32-column fp16 span
-        int rc = make_out_map(&mO, e.out, e.out_f32, e.ld_out, Nout, op->Xo, op->Yo, op->Zo, TW, TH, TN, e.out_f32 ? 32 : 64, "out");
-        if (rc) return rc;
-        mO2 = mO;
-        if (!e.out_f32 && !e.geglu) {
-            rc = make_out_map(&mO2, e.out, 0, e.ld_out, Nout, op->Xo, op->Yo, op->Zo, TW, TH, TN, 32, "out");
-            if (rc) return rc;
-        }
-        mR1 = mO; mR2 = mO;
-        if (e.res1) {
-            rc = make_out_map(&mR1, e.res1, e.res1_f32, e.ld_res1, op->N, op->Xo, op->Yo, op->Zo, TW, TH, TN, 32, "res1");
-            if (rc) return rc;
-        }
-        if (e.res2) {
-            rc = make_out_map(&mR2, e.res2, e.res2_f32, e.ld_res2, op->N, op->Xo, op->Yo, op->Zo, TW, TH, TN, 32, "res2");
-            if (rc) return rc;
-        }
-    }
     TmapSet ts;
-    ts.m[0] = mA; ts.m[1] = mB; ts.m[2] = mO; ts.m[3] = mO2; ts.m[4] = mR1; ts.m[5] = mR2;
+    ts.m[0] = mA; ts.m[1] = mB;
     tmap_cache_put(tkey, ts);
     }
-    // epilogue warpgroups: 2. Three (GCD_TC_NWG=3, experiments) measured 1-20 % SLOWER on every shape of tools/bench_ops.py
-    // (profiles/r2_notes.md §1): the third set of staging tiles costs pipeline stages and the 512-thread launch bound caps the
-    // epilogue at 128 registers, which serialises its eight independent polynomial chains.
-    const int NWG = nwg_cfg();
-    int rc = 0;
-    // (A K = 64-stage variant of the BN = 160 pair tiles for short-K ops with an fp32 residual — room for two residual tiles in
-    // flight per warpgroup, profiles/r1_notes.md §11 — measured SLOWER in situ: K=1280 5.44 -> 7.09 ms per 20 launches,
-    // profiles/r2_notes.md §3; not kept.)
-#define TC_GO(B, M) ((NWG == 3 && (rc = launch_tc<B, M, 3>(mA, mB, mO, mO2, mR1, mR2, p, st)) != TC_RETRY_NWG2) ? rc \
-                     : launch_tc<B, M, 2>(mA, mB, mO, mO2, mR1, mR2, p, st))
-    switch (BN * 10 + MODE) {
-        case 2563: rc = TC_GO(256, 3); break;
-        case 1604: rc = launch_tc<160, 4, 2>(mA, mB, mO, mO2, mR1, mR2, p, st); break;
-        case 1603: rc = TC_GO(160, 3); break;
-        case 1283: rc = TC_GO(128, 3); break;
-        case 2562: rc = TC_GO(256, 2); break;
-        case 1602: rc = TC_GO(160, 2); break;
-        case 1282: rc = TC_GO(128, 2); break;
-        case 2561: rc = TC_GO(256, 1); break;
-        case 1601: rc = TC_GO(160, 1); break;
-        default: rc = TC_GO(128, 1); break;
+    int rc;
+    switch (BN) {
+        case 256: rc = launch_tc<256>(mA, mB, p, st); break;
+        case 160: rc = launch_tc<160>(mA, mB, p, st); break;
+        default: rc = launch_tc<128>(mA, mB, p, st); break;
     }
-#undef TC_GO
     return rc ? rc : stats_skipped;
 }

@@ -148,8 +148,8 @@ static int gn_geometry(int64_t n_img, int64_t rows, int C, int groups, dim3* gri
     GCD_REQUIRE(C % 4 == 0 && C / 4 <= 1024, "groupnorm: C=%d unsupported", C);
     GCD_REQUIRE(groups > 0 && groups <= 64 && C % groups == 0 && (C / groups) % 2 == 0,
                 "groupnorm: C=%d groups=%d unsupported (need even channels per group, <=64 groups)", C, groups);
-    // ~256-thread blocks, ONE wave of them: the round-1 geometry (480-thread blocks, 48 registers -> 2 resident blocks = 47 %
-    // occupancy, two waves) ran gn_apply at 5.0 TB/s where layernorm_rows reaches 6.5 (profiles/r2_ncu_gn_apply.txt)
+    // ~256-thread blocks, ONE wave of them over the device's SMs (480-thread blocks at 48 registers leave 2 resident blocks =
+    // 47 % occupancy and two waves)
     int bx = C / 4;
     int by = 256 / bx;
     if (by < 1) by = 1;
@@ -158,7 +158,8 @@ static int gn_geometry(int64_t n_img, int64_t rows, int C, int groups, dim3* gri
     int per_sm = 1280 / threads;              // resident blocks per SM at <= 48 registers per thread (ptxas: 40-48)
     if (per_sm < 1) per_sm = 1;
     if (per_sm > 8) per_sm = 8;
-    int64_t want_blocks = (int64_t)148 * per_sm;
+    static const int num_sms = [] { int d = 0, n = 0; cudaGetDevice(&d); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d); return n > 0 ? n : 132; }();
+    int64_t want_blocks = (int64_t)num_sms * per_sm;
     int64_t chunks = want_blocks / (n_img > 0 ? n_img : 1);
     if (chunks < 1) chunks = 1;
     int64_t r = (rows + chunks - 1) / chunks;

@@ -36,7 +36,7 @@ class _EmbBase(_RefBase):
     @staticmethod
     def _need_cuda(x, who):
         if not x.is_cuda:
-            raise RuntimeError(f"gcd_b200.{who} runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError(f"gcd_b200.{who} runs on CUDA (sm_90a) only; there is no CPU path")
 
 
 class ConcatTimestepEmbedderND(_EmbBase):

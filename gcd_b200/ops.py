@@ -1,5 +1,5 @@
 """Thin torch-tensor front end over the C ABI (include/gcd_b200.h). Tensors are only used for device memory and the
-current CUDA stream; every op launches hand-written sm_100a kernels from libgcd_b200.so. No fallbacks."""
+current CUDA stream; every op launches hand-written sm_90a kernels from libgcd_b200.so. No fallbacks."""
 import ctypes
 
 import torch

@@ -1,11 +1,11 @@
-"""B200-native VideoUNet: drop-in for `sgm.modules.diffusionmodules.video_model.VideoUNet` (video_model.py:84-540).
+"""H100-native VideoUNet: drop-in for `sgm.modules.diffusionmodules.video_model.VideoUNet` (video_model.py:84-540).
 
 * `VideoUNet` is an nn.Module with the reference constructor kwargs, the reference `state_dict` keys/shapes
   (gcd_b200/spec.py) and the reference `forward` signature, so `instantiate_from_config` + `init_from_ckpt`
   (models/diffusion.py:76-79,191-219) work unchanged by switching the YAML `target:`.
 * `UNetEngine` is the execution plan underneath: weights repacked once to kernel-native fp16 layouts, activations kept
   channels-last `[frames, H*W, C]` (residual stream fp32, tensor-core operands 16-bit), every block executed by the
-  hand-written sm_100a kernels of libgcd_b200.so through gcd_b200.ops. There is no PyTorch compute fallback.
+  hand-written sm_90a kernels of libgcd_b200.so through gcd_b200.ops. There is no PyTorch compute fallback.
 
 Exact algebraic shortcuts taken (SURVEY.md §8(a) facts 1-5, all parity-tested against the oracle):
   - cross-attention context length is 1 in GCD => attn2(x, ctx) == to_out(to_v(ctx)): a per-frame (spatial) / per-clip
@@ -75,6 +75,14 @@ class BufferPool:
 
     def nbytes(self):
         return sum(b.numel() * b.element_size() for b in self.bufs.values())
+
+    def release(self, name):
+        """Drops the workspaces named `name` (their memory returns to the caching allocator)."""
+        self.bufs = {k: b for k, b in self.bufs.items() if k[0] != name}
+
+    def release_rows(self, rows):
+        """Drops the workspaces whose leading dimension is `rows` (their memory returns to the caching allocator)."""
+        self.bufs = {k: b for k, b in self.bufs.items() if k[1][:1] != (rows,)}
 
 
 class StatsArena:
@@ -581,7 +589,7 @@ class VideoUNet(nn.Module):
     def forward(self, x, timesteps, context=None, y=None, time_context=None, num_video_frames=None,
                 image_only_indicator=None):
         if not x.is_cuda:
-            raise RuntimeError("gcd_b200.VideoUNet runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("gcd_b200.VideoUNet runs on CUDA (sm_90a) only; there is no CPU path")
         if time_context is not None:
             raise NotImplementedError("time_context must be None (use_spatial_context=True derives it from context)")
         if image_only_indicator is not None and bool((image_only_indicator != 0).any()):

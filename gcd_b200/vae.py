@@ -1,4 +1,4 @@
-"""B200-native temporal VAE decoder: drop-in for `sgm.modules.autoencoding.temporal_ae.VideoDecoder`
+"""H100-native temporal VAE decoder: drop-in for `sgm.modules.autoencoding.temporal_ae.VideoDecoder`
 (temporal_ae.py:293-349 over diffusionmodules/model.py:604-748), time_mode "conv-only" (the default, :302).
 
 `DiffusionEngine.decode_first_stage` gates on `isinstance(decoder, VideoDecoder)` (models/diffusion.py:242,620), so
@@ -7,8 +7,8 @@ __init__ is bypassed); standalone it is a plain nn.Module. State-dict keys equal
 (`first_stage_model.decoder.*`, gcd_b200/spec.py).
 
 Execution: channels-last, fp32 residual stream, 16-bit tensor-core operands, all compute in libgcd_b200.so kernels:
-3x3 / (3,1,1) convs = tcgen05 implicit GEMM with fused bias/residual/alpha-blend epilogues, GroupNorm+SiLU streaming
-kernels, the single-head d=512 mid attention as batched tcgen05 GEMMs (QK^T, PV) + a row-softmax kernel.
+3x3 / (3,1,1) convs = wgmma implicit GEMM with fused bias/residual/alpha-blend epilogues, GroupNorm+SiLU streaming
+kernels, the single-head d=512 mid attention as batched wgmma GEMMs (QK^T, PV) + a row-softmax kernel.
 """
 import torch
 import torch.nn as nn
@@ -174,11 +174,16 @@ class DecoderEngine:
             elif kind == "up":
                 xu = pool.get(f"up{cin}_{rows * 4}", (rows * 4, cin), AD)
                 ops.upsample2x_to_act(h, n, hH, hW, cin, xu)
+                # the lower level's workspaces are dead from here on: free them, so that the decoder's peak is its largest
+                # level alone (14 frames at 576x1024 px would otherwise hold every level's buffers at once, ~55 GB)
+                pool.release_rows(rows)
                 hH, hW = 2 * hH, 2 * hW
                 h = pool.get(f"s0_{cout}_{rows * 4}", (rows * 4, cout), torch.float32)
                 st, req = self._stats_req(n, cout, hH * hW)
                 ok = ops.conv2d_3x3(xu.view(n, hH, hW, cin), W[p + ".w"], ops.make_ep(h, bias=W[p + ".b"], gn_stats=req))
                 hst = st if ok else None
+                pool.release(f"up{cin}_{rows * 4}")            # the upsampled input is dead once the conv has read it
+                del xu
             elif kind == "out":
                 a = pool.get(f"a{cin}_{rows}", (rows, cin), AD)
                 self._gn(h, n, hH * hW, cin, "norm_out", 1e-6, True, a, stats=hst)
@@ -343,7 +348,7 @@ class Encoder(nn.Module):
 
     def _run(self, x, eng):
         if not x.is_cuda:
-            raise RuntimeError("gcd_b200.Encoder runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("gcd_b200.Encoder runs on CUDA (sm_90a) only; there is no CPU path")
         n, c, H, W = x.shape
         ndown = len(self.cfg["ch_mult"]) - 1
         if c != self.cfg["in_channels"] or H % (1 << ndown) or W % (1 << ndown) or ((H >> ndown) * (W >> ndown)) % 8:
@@ -421,7 +426,7 @@ class VideoDecoder(_Base):
     @torch.no_grad()
     def forward(self, z, timesteps=None, skip_video=False, **kwargs):
         if not z.is_cuda:
-            raise RuntimeError("gcd_b200.VideoDecoder runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("gcd_b200.VideoDecoder runs on CUDA (sm_90a) only; there is no CPU path")
         if skip_video or timesteps is None:
             raise NotImplementedError("VideoDecoder needs timesteps=<frames per clip> and skip_video=False")
         n, c, H, W = z.shape

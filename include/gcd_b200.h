@@ -1,4 +1,4 @@
-/* gcd_b200 — C ABI of the B200-native GCD denoising hot path.
+/* gcd_b200 — C ABI of the H100-native (sm_90a) GCD denoising hot path.
  *
  * The reference (basilevh/gcd, gcd-model/sgm) is pure Python/PyTorch and has NO FFI of its own
  * (SURVEY.md §8(b)); the drop-in boundary upstream is the `instantiate_from_config` plugin surface
@@ -62,7 +62,7 @@ typedef struct gcd_epilogue {
     int64_t gn_rows_per_img;
 } gcd_epilogue;
 
-/* Generic tcgen05 implicit-GEMM:  acc[r, n] = sum_{tap, c} A[(x,y,z)(r) * in_mul + tap_off(tap), c] * W[n, tap*Cin + c]
+/* Generic wgmma implicit-GEMM:  acc[r, n] = sum_{tap, c} A[(x,y,z)(r) * in_mul + tap_off(tap), c] * W[n, tap*Cin + c]
  * A is a 4-D channels-last act tensor (C innermost, then X, Y, Z) with element strides; out-of-range
  * coordinates read as zero (= conv zero padding). Output rows are (z*Yo + y)*Xo + x.
  * Replaces nn.Linear / nn.Conv2d(3x3, 1x1, stride 1|2) / nn.Conv3d((3,1,1)) / torch.bmm on the hot path. */
@@ -164,8 +164,8 @@ int gcd_sampler_prep(const float* x, const float* uc_concat, const float* c_conc
 int gcd_sampler_update(float* x, const float* net_out, int ld_net, int BT, int T, int H, int W, float c_out,
                        float c_skip, float sigma, float dt, const float* scale, void* stream);
 
-/* Experiments only (tools/autotune_tc.py): force tile width (128 / 160 / 256) and cluster mode (2 = weight multicast, 3 = CTA-pair
- * MMA) of the following gcd_tc_run calls; 0 = automatic. Not thread-safe. */
+/* Experiments only (tools/autotune_tc.py): force the tile width (128 / 160 / 256) of the following gcd_tc_run calls; 0 = automatic.
+ * `mode` is ignored (kept for ABI compatibility). Not thread-safe. */
 void gcd_tc_override(int bn, int mode);
 
 /* Evaluation-loop image metrics (gcd-model/scripts/test.py:346-496 calculate_metrics; SSIM = scikit-image 0.22.0

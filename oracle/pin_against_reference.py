@@ -1,4 +1,4 @@
-"""Pins the oracle to the reference and writes tests/golden/ (run in the BUILD CONTAINER only; needs /root/reference).
+"""Pins the oracle to the reference and writes tests/golden/ (needs a reference checkout: GCD_REFERENCE, see oracle/ref_shim.py).
 
     python -m oracle.pin_against_reference [--full]
 
@@ -140,6 +140,50 @@ def pin_embedders():
     torch.save(out, os.path.join(GOLD, "embedders.pt"))
 
 
+def pin_ema_and_conditioner():
+    """What the reference's LitEma (modules/ema.py) and GeneralConditioner (encoders/modules.py:93-96) make of this package's
+    modules, stored as JSON so that the tests need neither the reference tree nor its dependencies."""
+    import json
+    import types
+    ref_shim.install()
+    from sgm.modules.ema import LitEma
+    from gcd_b200 import checkpoint, spec
+    from gcd_b200.unet import VideoUNet
+    from gcd_b200.vae import Encoder, VideoDecoder
+    net = VideoUNet(**spec.unet_ctor_kwargs(UNET_TINY))
+    root = checkpoint.HotPathRoot(VideoUNet(**spec.unet_ctor_kwargs(UNET_TINY)),
+                                  VideoDecoder(**spec.decoder_ctor_kwargs(VAE_TINY)),
+                                  Encoder(**spec.encoder_ctor_kwargs(spec.VAE_ENCODER_TINY)))
+    out = {"litema_unet_tiny": dict(sorted(LitEma(net, decay=0.999).m_name2s_name.items())),
+           "litema_root_model_buffers": sorted(n for n, _ in LitEma(root.model, decay=0.999).named_buffers())}
+    # GeneralConditioner over the two embedders, with the reference's own AbstractEmbModel as their base class
+    ast_ns = ref_shim.conditioner_classes()
+    fake = types.ModuleType("sgm.modules.encoders.modules")
+    fake.AbstractEmbModel, fake.GeneralConditioner = ast_ns["AbstractEmbModel"], ast_ns["GeneralConditioner"]
+    pkg = types.ModuleType("sgm.modules.encoders")
+    pkg.__path__ = []
+    sys.modules["sgm.modules.encoders"], sys.modules["sgm.modules.encoders.modules"] = pkg, fake
+    import importlib
+    import gcd_b200.embedders as E
+    E = importlib.reload(E)
+    cond = fake.GeneralConditioner(CONDITIONER_EMBEDDERS)
+    out["conditioner"] = {"config": CONDITIONER_EMBEDDERS, "input_keys": [e.input_key for e in cond.embedders], "ucg_rate": [e.ucg_rate for e in cond.embedders],
+                          "is_trainable": [e.is_trainable for e in cond.embedders],
+                          "classes": [type(e).__name__ for e in cond.embedders]}
+    import gzip
+    with gzip.open(os.path.join(GOLD, "ref_ema_conditioner.json.gz"), "wt") as f:
+        json.dump(out, f, separators=(",", ":"))
+    print(f"[ema / conditioner] {len(out['litema_unet_tiny'])} LitEma shadows; conditioner {out['conditioner']}")
+
+
+# the conditioner entries of the GCD configs that this package replaces (infer_kubric.yaml), as GeneralConditioner input
+CONDITIONER_EMBEDDERS = [
+    {"target": "gcd_b200.embedders.ConcatTimestepEmbedderND", "params": {"outdim": 256}, "input_key": "fps_id",
+     "is_trainable": False},
+    {"target": "gcd_b200.embedders.SphericalEmbedder", "params": {"embed_dim": 128}, "input_key": "spherical",
+     "is_trainable": False, "ucg_rate": 0.1}]
+
+
 def pin_closed_forms():
     """Known-answer values derivable from the source (SURVEY.md §8(c))."""
     ref_shim.install()
@@ -168,6 +212,7 @@ if __name__ == "__main__":
     pin_decoder("tiny", VAE_TINY, T=3, H=8, W=8)
     pin_encoder("tiny", dict(O.VAE_ENCODER, ch=64), n=2, H=64, W=96)
     pin_embedders()
+    pin_ema_and_conditioner()
     if "--full" in sys.argv:
         pin_unet("kubric", O.UNET_KUBRIC, B=1, T=2, H=16, W=16, steps=2)
         pin_unet("pardom", O.UNET_PARDOM, B=1, T=2, H=8, W=8, steps=1)

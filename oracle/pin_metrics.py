@@ -19,7 +19,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import metrics_oracle as M  # noqa: E402
 
-REF = "/root/reference/gcd-model/scripts/eval_utils.py"
+REF = os.path.join(os.environ.get("GCD_REFERENCE", ""), "scripts", "eval_utils.py")
 
 
 def _stub_skimage():

@@ -1,4 +1,6 @@
-"""Imports the reference's own hot-path modules from /root/reference (build container only; TEST INFRASTRUCTURE).
+"""Imports the reference's own hot-path modules from a checkout of basilevh/gcd (TEST INFRASTRUCTURE: only the scripts that
+write tests/golden/ use it; the tests themselves read the stored goldens). Point GCD_REFERENCE at the checkout's `gcd-model`
+directory.
 
 `import sgm` fails upstream (needs pytorch_lightning / omegaconf / open_clip / kornia, absent here — SURVEY.md §8(c)),
 so empty package shells named `sgm`, `sgm.modules`, `sgm.models` are pre-registered with __path__ pointing at the
@@ -8,18 +10,18 @@ import os
 import sys
 import types
 
-REF = "/root/reference/gcd-model"
+REF = os.environ.get("GCD_REFERENCE", "")
 
 
 def available():
-    return os.path.isdir(os.path.join(REF, "sgm"))
+    return bool(REF) and os.path.isdir(os.path.join(REF, "sgm"))
 
 
 def install():
     if "sgm" in sys.modules and getattr(sys.modules["sgm"], "_gcd_shim", False):
         return
     if not available():
-        raise RuntimeError("reference tree not present (only available in the build container)")
+        raise RuntimeError("reference tree not found: set GCD_REFERENCE to the gcd-model directory of a basilevh/gcd checkout")
     for name, sub in (("sgm", "sgm"), ("sgm.modules", "sgm/modules"), ("sgm.models", "sgm/models"),
                       ("sgm.modules.autoencoding", "sgm/modules/autoencoding"),
                       ("sgm.modules.diffusionmodules", "sgm/modules/diffusionmodules")):
@@ -107,3 +109,23 @@ def ref_embedder_classes():
     ns = {"torch": torch, "nn": nn, "rearrange": rearrange, "Timestep": Timestep, "Union": __import__("typing").Union}
     exec(compile(ast.Module(body=body, type_ignores=[]), path, "exec"), ns)
     return ns["ConcatTimestepEmbedderND"], ns["SphericalEmbedder"]
+
+
+def conditioner_classes():
+    """The reference's AbstractEmbModel and GeneralConditioner. Their module cannot be imported here (open_clip / kornia), so
+    the two class definitions are cut out of the reference source with `ast` and executed."""
+    install()
+    import ast
+    import typing
+    import torch
+    import torch.nn as nn
+    from gcd_b200.sampling import instantiate_from_config
+    path = os.path.join(REF, "sgm", "modules", "encoders", "modules.py")
+    tree = ast.parse(open(path).read())
+    body = [n for n in tree.body if isinstance(n, ast.ClassDef) and n.name in ("AbstractEmbModel", "GeneralConditioner")]
+    assert len(body) == 2
+    ns = {"torch": torch, "nn": nn, "Union": typing.Union, "List": typing.List, "Dict": typing.Dict, "Optional": typing.Optional,
+          "ListConfig": list, "instantiate_from_config": instantiate_from_config, "disabled_train": lambda self, mode=True: self,
+          "count_params": lambda m, verbose=False: 0, "print": lambda *a, **k: None}
+    exec(compile(ast.Module(body=body, type_ignores=[]), path, "exec"), ns)
+    return ns

@@ -7,6 +7,9 @@ traj50.pt, vae_fullres.pt — written by oracle/pin_metric_shape.py in the build
 * the complete 25-step Euler trajectory at 14x32x48, full width (BASELINE.md §4.4), and the 50-step / max-scale-2.5 one of
   BASELINE config 4 at 14x16x24, intermediate states included;
 * the VideoDecoder at 576x1024 px (14 frames), against a strided subsample, full-resolution crops and per-frame moments;
+
+The network outputs and trajectory states are stored as fixed strided subsamples (rows 2, columns 4 / columns 2) to keep the
+fixtures small; every sampled element is compared.
 * the sigma schedule the product puts on the DEVICE, bit for bit against the reference's values.
 
 Stated tolerances (relative L2 vs the fp32 reference; 16-bit tensor-core operands, fp32 accumulate / residual / norms):
@@ -34,7 +37,7 @@ def relerr(a, b):
 def _gold(name):
     path = os.path.join(GOLD, name)
     if not os.path.exists(path):
-        pytest.skip(f"{name} not generated (oracle/pin_metric_shape.py, build container)")
+        pytest.skip(f"{name} not generated (oracle/pin_metric_shape.py)")
     return torch.load(path)
 
 
@@ -84,9 +87,10 @@ def test_unet_forward_at_metric_shape_vs_reference(tag):
     xin = torch.cat((torch.cat([x, x]) * gold["x_mul"] * ci, c_cat["concat"]), 1)
     out = net(xin.cuda(), cn.reshape(-1).cuda(), context=c_cat["crossattn"].cuda(), y=c_cat["vector"].cuda(),
               num_video_frames=T, image_only_indicator=ioi.cuda())
-    assert out.shape == gold["net_out"].shape
-    e = relerr(out, gold["net_out"])
-    worst = max(relerr(out[f], gold["net_out"][f]) for f in range(2 * T))
+    assert out.shape == (2 * T, 4, H, W)
+    out = out[:, :, ::2, ::4]                           # the stored subsample
+    e = relerr(out, gold["net_out_sub"])
+    worst = max(relerr(out[f], gold["net_out_sub"][f]) for f in range(2 * T))
     print(f"unet[{tag}] 28x72x128 rel-L2 vs reference: {e:.3e} (worst frame {worst:.3e})")
     assert e < TOL_NET and worst < 2 * TOL_NET
 
@@ -117,8 +121,9 @@ def test_full_trajectory_vs_reference(name):
     """The whole sampler loop (sampling.py:123-144): state after selected step counts and the final sample."""
     gold = _gold(f"{name}.pt")
     out, trace = _sample(gold)
-    errs = {k: relerr(trace[k], v) for k, v in sorted(gold["after_steps"].items()) if k in trace}
-    e = relerr(out, gold["sampled"])
+    ws = gold.get("w_stride", 1)                        # stored states: every ws-th latent column
+    errs = {k: relerr(trace[k][..., ::ws], v) for k, v in sorted(gold["after_steps"].items()) if k in trace}
+    e = relerr(out[..., ::ws], gold["sampled"])
     print(f"{name}: {gold['steps']} steps at 14x{gold['H']}x{gold['W']}, max scale {gold['max_scale']}: rel-L2 after k steps "
           f"{ {k: f'{v:.2e}' for k, v in errs.items()} }, final {e:.3e}")
     assert len(errs) >= 3 and all(v < TOL_SAMPLE for v in errs.values())
@@ -140,7 +145,7 @@ def test_vae_decode_full_resolution_vs_reference():
     z = torch.randn(T, cfg["z_channels"], H, W, generator=g)
     out = dec((z / 0.18215).cuda(), timesteps=T)
     assert out.shape == (T, 3, 8 * H, 8 * W)
-    e_sub = relerr(out[:, :, ::8, ::8], gold["sub8"])
+    e_sub = relerr(out[:, :, ::16, ::16], gold["sub16"])
     e_crop = max(relerr(out[f, :, y0:y0 + 64, x0:x0 + 64], cr) for (f, y0, x0), cr in zip(gold["crop_pos"], gold["crops"]))
     e_mean = (out.mean(dim=(2, 3)).cpu() - gold["mean"]).abs().max().item() / gold["sqmean"].sqrt().max().item()
     e_sq = relerr(out.pow(2).mean(dim=(2, 3)), gold["sqmean"])

@@ -1,4 +1,4 @@
-"""Autotune study of `tc_gemm_kernel`'s tile width / cluster mode per op of the hot path (experiments; B200 via gpurun).
+"""Autotune study of `tc_gemm_kernel`'s tile width / cluster mode per op of the hot path (experiments, on an H100; the cluster-mode argument is ignored by the Hopper kernel).
 
 Records every `gcd_tc_run` descriptor of one full-size CFG forward + one VAE decode, then re-issues each DISTINCT op (same buffers,
 same fused epilogue) under every (BN, mode) the kernel supports — `gcd_tc_override` — and times it with CUDA events (median of 7,

@@ -1,4 +1,4 @@
-"""Micro-benchmarks of the hot kernels at the BASELINE shapes (config 5): run on the B200 via gpurun."""
+"""Micro-benchmarks of the hot kernels at the BASELINE shapes (config 5): run on an H100."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

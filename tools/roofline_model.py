@@ -1,8 +1,8 @@
 """Per-shape bound model of the tensor-core ops of one CFG forward, against the CUDA-event times of tools/prof_forward.py
-(default input profiles/r2_prof_forward_final.txt; `python tools/roofline_model.py <file>` for another record).
+(`python tools/roofline_model.py <file>` with the output of tools/prof_forward.py).
 
 For every `tc M.. N.. K..` line: time at the tensor bound (measured burst bf16 peak), at the L2->SM operand-traffic bound (TMA chip
-throughput ~6 300 B/clk ~ 11 TB/s, see profiles/r1_notes.md §8) and at the HBM bound (algorithmic bytes / measured copy peak),
+throughput) and at the HBM bound (algorithmic bytes / measured copy peak),
 using the same tile policy as gcd_tc_run (BN 256/160/128, CTA pair for long K, weight multicast for short K)."""
 import json, os, re, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

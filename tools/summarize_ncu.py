@@ -1,7 +1,7 @@
-"""Turn ncu outputs brought back in gpurun_out/ into the small text/CSV summaries committed under profiles/.
+"""Turn ncu outputs into small text/CSV summaries.
 
-  python tools/summarize_ncu.py launches gpurun_out/launches.csv profiles/r1_launches_summary.csv
-  python tools/summarize_ncu.py full gpurun_out/prof_conv.ncu-rep profiles/r1_ncu_prof_conv.txt [kernel-substring]
+  python tools/summarize_ncu.py launches launches.csv launches_summary.csv
+  python tools/summarize_ncu.py full prof_conv.ncu-rep ncu_prof_conv.txt [kernel-substring]
 """
 import csv, io, re, subprocess, sys
 from collections import defaultdict

@@ -1,5 +1,5 @@
 // Micro-benchmark: MUFU ex2 throughput per SM for f32, f16x2 and bf16x2 operands (is the packed form 2 exps per lane-op?).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench/mufu tools/ubench/mufu.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench/mufu tools/ubench/mufu.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -22,9 +22,9 @@ __global__ void k(float* out, int iters, float seed) {
     out[blockIdx.x * blockDim.x + threadIdx.x] = a0 + a1 + a2 + a3 + __uint_as_float(h0 ^ h1 ^ h2 ^ h3);
 }
 int main() {
-    float* out; cudaMalloc(&out, 148 * 8 * 1024 * 4);
+    float* out; cudaMalloc(&out, 132 * 8 * 1024 * 4);
     int clk; cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0);
-    const int iters = 20000, blocks = 148 * 2, threads = 1024;
+    const int iters = 20000, blocks = 132 * 2, threads = 1024;
     const char* names[3] = {"ex2.f32", "ex2.f16x2", "ex2.bf16x2"};
     for (int m = 0; m < 3; m++) {
         cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
@@ -38,7 +38,7 @@ int main() {
         float ms; cudaEventElapsedTime(&ms, e0, e1);
         double instr = (double)blocks * threads * iters * 4;
         printf("%-10s %.3f ms  %.2f lane-instr/ns chip = %.1f lane-instr/clk/SM at max clock %d MHz (x2 values for packed)\n", names[m], ms,
-               instr / (ms * 1e6), instr / (ms * 1e-3) / 148 / (clk * 1e3), clk / 1000);
+               instr / (ms * 1e6), instr / (ms * 1e-3) / 132 / (clk * 1e3), clk / 1000);
     }
     printf("err %s\n", cudaGetErrorString(cudaGetLastError()));
     return 0;
