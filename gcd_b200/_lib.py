@@ -49,7 +49,12 @@ _SIGS = {
                                     c_float, c_int, c_void_p, c_void_p]),
     "gcd_layernorm": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_float, c_void_p, c_int64, c_int64,
                               c_void_p, c_void_p, c_void_p]),
+    "gcd_layernorm_f32": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_float, c_void_p, c_int64, c_int64,
+                                  c_void_p, c_void_p]),
     "gcd_attention_spatial": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "gcd_attention_d80": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "gcd_clip_preprocess": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                    c_void_p, c_int, c_void_p]),
     "gcd_attention_temporal": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "gcd_softmax_rows": (c_int, [c_void_p, c_int64, c_int, c_float, c_void_p, c_void_p]),
     "gcd_memset_async": (c_int, [c_void_p, c_int, c_int64, c_void_p]),
@@ -72,12 +77,18 @@ _SIGS = {
 }
 
 EXPORTS = tuple(_SIGS.keys())
+MISSING = []      # declared symbols the loaded library does not export (a GCD_LIB_PATH build of older sources)
 
 _lib = None
 
 
 def load():
-    """Loads the shared library (once). Raises GcdError if it has not been built (python -m gcd_b200.build)."""
+    """Loads the shared library (once). Raises GcdError if it has not been built (python -m gcd_b200.build).
+
+    A declared symbol the library does not export is left unbound and listed in MISSING: calling it raises AttributeError
+    (undefined symbol), while everything the library does export works. That keeps a variant build of older sources usable
+    through GCD_LIB_PATH for the paths it covers (A/B of the sampler against an earlier library); the in-tree build exports
+    every symbol (checked by build() and tests/test_host_cpu.py)."""
     global _lib
     if _lib is not None:
         return _lib
@@ -85,8 +96,13 @@ def load():
         raise GcdError(f"{LIB_PATH} is missing: build it with `python -m gcd_b200.build` "
                        "(gcd_b200 has no CPU / eager fallback)")
     lib = ctypes.CDLL(LIB_PATH)
+    MISSING.clear()
     for name, (res, args) in _SIGS.items():
-        fn = getattr(lib, name)  # AttributeError if a declared symbol is not exported
+        try:
+            fn = getattr(lib, name)
+        except AttributeError:
+            MISSING.append(name)
+            continue
         fn.restype = res
         fn.argtypes = args
     _lib = lib

@@ -125,7 +125,10 @@ __device__ __forceinline__ float2 ld_res2(const void* base, bool f32, int64_t of
 //                 batch in flight while the previous stage is released), then the fused epilogue straight from the
 //                 accumulator registers: bias (+ per-row vector) / SiLU / scale / GEGLU / two residual blends, 16-bit or fp32
 //                 stores, and the GroupNorm statistics of the stored values.
-template <int BN>
+// GELU: the `act == 2` (exact erf GELU) instantiation. Kept out of the act 0 / 1 kernels: the erff expansion inside their
+// unrolled epilogue made the UNet's tc_gemm 14 % slower (same registers; one H100 80GB HBM3 at 400 W). The act 0 / 1
+// instantiations compile to the same SASS as without GELU.
+template <int BN, bool GELU>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const TcParams p) {
     constexpr int B_BYTES = BN * 128;
@@ -290,7 +293,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     if (grow[h] < 0) continue;
                     float v0 = acc[4 * i + 2 * h] + b.x, v1 = acc[4 * i + 2 * h + 1] + b.y;
                     if (rv[h]) { v0 += rv[h][col]; if (c1ok) v1 += rv[h][col + 1]; }
-                    if (p.act == 1) { v0 = silu(v0); v1 = silu(v1); }
+                    if constexpr (GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+                    else if (p.act == 1) { v0 = silu(v0); v1 = silu(v1); }
                     v0 *= p.a0; v1 *= p.a0;
                     if (p.res1) {
                         const int64_t o = grow[h] * p.ld1 + col;
@@ -366,11 +370,11 @@ static int num_sms_cached() {
     return n;
 }
 
-template <int BN>
+template <int BN, bool GELU>
 static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, TcParams& p, cudaStream_t st) {
     static bool configured = false;
     if (!configured) {
-        GCD_CUDA_CHECK(cudaFuncSetAttribute(tc_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
+        GCD_CUDA_CHECK(cudaFuncSetAttribute(tc_gemm_kernel<BN, GELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
         configured = true;
     }
     constexpr int STAGE_BYTES = TC_A_BYTES + BN * 128;
@@ -384,7 +388,7 @@ static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, TcParams& p, 
     const int sms = num_sms_cached();
     GCD_REQUIRE(sms > 0, "tc_gemm: no CUDA device");
     const int grid = tiles < sms ? tiles : sms;
-    tc_gemm_kernel<BN><<<grid, TC_THREADS, smem, st>>>(mA, mB, p);
+    tc_gemm_kernel<BN, GELU><<<grid, TC_THREADS, smem, st>>>(mA, mB, p);
     GCD_CUDA_CHECK(cudaGetLastError());
     g_launches++;
     return 0;
@@ -441,6 +445,7 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
     const gcd_epilogue& e = op->ep;
     GCD_REQUIRE(!e.geglu || (op->N % 256 == 0 && !e.out_f32 && !e.res1 && !e.res2 && e.a_acc == 1.0f && !e.act),
                 "gcd_tc_run: GEGLU needs N %% 256 == 0, 16-bit output, no residual / scale / activation");
+    GCD_REQUIRE(e.act >= 0 && e.act <= 2, "gcd_tc_run: act=%d unsupported (0 none, 1 SiLU, 2 GELU)", e.act);
     GCD_REQUIRE(!e.rowvec || e.rows_per_vec > 0, "gcd_tc_run: rows_per_vec must be > 0");
     GCD_REQUIRE(!e.bias || ((uintptr_t)e.bias & 15) == 0, "gcd_tc_run: bias must be 16B aligned");
     GCD_REQUIRE(!e.rowvec || (((uintptr_t)e.rowvec & 15) == 0 && e.ld_rowvec % 4 == 0),
@@ -555,9 +560,9 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
     }
     int rc;
     switch (BN) {
-        case 256: rc = launch_tc<256>(mA, mB, p, st); break;
-        case 160: rc = launch_tc<160>(mA, mB, p, st); break;
-        default: rc = launch_tc<128>(mA, mB, p, st); break;
+        case 256: rc = e.act == 2 ? launch_tc<256, true>(mA, mB, p, st) : launch_tc<256, false>(mA, mB, p, st); break;
+        case 160: rc = e.act == 2 ? launch_tc<160, true>(mA, mB, p, st) : launch_tc<160, false>(mA, mB, p, st); break;
+        default: rc = e.act == 2 ? launch_tc<128, true>(mA, mB, p, st) : launch_tc<128, false>(mA, mB, p, st); break;
     }
     return rc ? rc : stats_skipped;
 }

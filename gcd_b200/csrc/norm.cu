@@ -244,10 +244,11 @@ extern "C" int gcd_groupnorm_apply(const void* in, int in_f32, int64_t n_img, in
 // ---------------------------------------------------------------------------------------------- LayerNorm
 // One warp per row; the row (<= 2048 channels) lives in registers: mean, then centred variance (two-pass, fp32).
 constexpr int LN_MAXK = 32;  // float2 per lane -> C <= 2048
+template <typename OutT>     // act_t, or float for a normalised tensor that is itself a residual stream (gcd_layernorm_f32)
 __global__ void layernorm_kernel(const float* __restrict__ in, int64_t rows, int C, const float* __restrict__ gamma,
                                  const float* __restrict__ beta, float eps, const float* __restrict__ add,
                                  int64_t add_rows_per, int64_t add_mod, float* __restrict__ sum_out,
-                                 act_t* __restrict__ out) {
+                                 OutT* __restrict__ out) {
     const int lane = threadIdx.x & 31;
     const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= rows) return;
@@ -287,12 +288,13 @@ __global__ void layernorm_kernel(const float* __restrict__ in, int64_t rows, int
     const float rstd = rsqrtf(q / (float)C + eps);
     const float2* g2 = reinterpret_cast<const float2*>(gamma);
     const float2* b2 = reinterpret_cast<const float2*>(beta);
-    uint32_t* dst = reinterpret_cast<uint32_t*>(out + row * C);
 #pragma unroll
     for (int k = 0; k < LN_MAXK; k++) {
         if (k < nk) {
             float2 g = __ldg(&g2[lane + 32 * k]), b = __ldg(&b2[lane + 32 * k]);
-            dst[lane + 32 * k] = pack2((v[k].x - mean) * rstd * g.x + b.x, (v[k].y - mean) * rstd * g.y + b.y);
+            const float y0 = (v[k].x - mean) * rstd * g.x + b.x, y1 = (v[k].y - mean) * rstd * g.y + b.y;
+            if constexpr (sizeof(OutT) == 4) reinterpret_cast<float2*>(out + row * C)[lane + 32 * k] = make_float2(y0, y1);
+            else reinterpret_cast<uint32_t*>(out + row * C)[lane + 32 * k] = pack2(y0, y1);
         }
     }
 }
@@ -398,9 +400,25 @@ extern "C" int gcd_layernorm(const float* in, int64_t rows, int C, const float* 
     }
     const int warps = 8;
     int64_t blocks = (rows + warps - 1) / warps;
-    layernorm_kernel<<<(unsigned)blocks, warps * 32, 0, (cudaStream_t)stream>>>(in, rows, C, gamma, beta, eps, add,
-                                                                                add_rows_per, add_mod, sum_out,
-                                                                                (act_t*)out);
+    layernorm_kernel<act_t><<<(unsigned)blocks, warps * 32, 0, (cudaStream_t)stream>>>(in, rows, C, gamma, beta, eps, add,
+                                                                                       add_rows_per, add_mod, sum_out,
+                                                                                       (act_t*)out);
+    GCD_CUDA_CHECK(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+// The same LayerNorm with a float32 output: the ViT's ln_pre output is the residual stream itself (open_clip
+// VisionTransformer.forward: x = ln_pre(x + positional_embedding), then x = x + attn(ln_1(x)) ...), so it stays fp32.
+extern "C" int gcd_layernorm_f32(const float* in, int64_t rows, int C, const float* gamma, const float* beta, float eps,
+                                 const float* add, int64_t add_rows_per, int64_t add_mod, float* out, void* stream) {
+    GCD_REQUIRE(C % 64 == 0 && C <= 64 * LN_MAXK, "layernorm_f32: C=%d must be a multiple of 64 and <= %d", C, 64 * LN_MAXK);
+    GCD_REQUIRE(!add || (add_rows_per > 0 && add_mod > 0), "layernorm_f32: bad add indexing");
+    GCD_REQUIRE(out != in, "layernorm_f32: out must not alias in");
+    const int warps = 8;
+    const int64_t blocks = (rows + warps - 1) / warps;
+    layernorm_kernel<float><<<(unsigned)blocks, warps * 32, 0, (cudaStream_t)stream>>>(in, rows, C, gamma, beta, eps, add,
+                                                                                       add_rows_per, add_mod, nullptr, out);
     GCD_CUDA_CHECK(cudaGetLastError());
     g_launches++;
     return 0;

@@ -245,6 +245,16 @@ def layernorm(x, gamma, beta, out, eps=1e-5, add=None, add_rows_per=1, add_mod=1
                                   int(add_mod), _p(sum_out), _p(out), _stream()), "layernorm")
 
 
+def layernorm_f32(x, gamma, beta, out, eps=1e-5, add=None, add_rows_per=1, add_mod=1):
+    """LayerNorm written as float32 (the ViT's ln_pre, whose output is the residual stream)."""
+    _need_cuda(x, gamma, beta, out, add)
+    rows, C = x.shape
+    assert x.dtype == torch.float32 and x.is_contiguous() and out.dtype == torch.float32 and out.is_contiguous()
+    with _timed("layernorm", 0.0, rows * C * 8):
+        check(lib().gcd_layernorm_f32(_p(x), rows, C, _p(gamma), _p(beta), float(eps), _p(add), int(add_rows_per),
+                                      int(add_mod), _p(out), _stream()), "layernorm_f32")
+
+
 def softmax_rows(x, scale, out):
     _need_cuda(x, out)
     rows, cols = x.shape
@@ -266,6 +276,31 @@ def attention_temporal(qkv, clips, T, tokens, heads, out):
     assert qkv.dtype == act_dtype() and qkv.is_contiguous() and out.is_contiguous()
     with _timed("attn_temporal", 4.0 * clips * tokens * heads * T * T * 64, clips * T * tokens * heads * 64 * 8):
         check(lib().gcd_attention_temporal(_p(qkv), clips, T, tokens, heads, _p(out), _stream()), "attention_temporal")
+
+
+def attention_d80(qkv, n, L, heads, out):
+    """qkv: act [n*L, 3*heads*80] (q | k | v) -> out act [n*L, heads*80] (ViT self-attention, head_dim 80)."""
+    _need_cuda(qkv, out)
+    assert qkv.dtype == act_dtype() and qkv.is_contiguous() and out.is_contiguous()
+    assert qkv.shape == (n * L, 3 * heads * 80) and out.shape == (n * L, heads * 80)
+    with _timed("attn_d80", 4.0 * n * heads * L * L * 80, n * L * heads * 80 * 8):
+        check(lib().gcd_attention_d80(_p(qkv), n, L, heads, _p(out), _stream()), "attention_d80")
+
+
+def clip_preprocess(x, taps_x, taps_y, mean_std, out, scratch=None):
+    """x: float32 NCHW [n, 3, H, W] in [-1, 1] -> out [n*257, 640] patch matrix, act or float32 (include/gcd_b200.h). taps_*: float32
+    device tensors of odd length, or None for no antialias blur; scratch: float32 [2*n*3*H*W] when blurring."""
+    _need_cuda(x, taps_x, taps_y, mean_std, out, scratch)
+    n, c, H, W = x.shape
+    assert c == 3 and x.dtype == torch.float32 and x.is_contiguous()
+    assert out.shape == (n * 257, 640) and out.is_contiguous()
+    ks_x = 0 if taps_x is None else taps_x.numel()
+    ks_y = 0 if taps_y is None else taps_y.numel()
+    if ks_x:
+        assert scratch is not None and scratch.dtype == torch.float32 and scratch.numel() >= 2 * x.numel()
+    with _timed("elem", 0.0, x.numel() * (4 + (16 if ks_x else 0)) + out.numel() * 2):
+        check(lib().gcd_clip_preprocess(_p(x), n, H, W, _p(taps_x), ks_x, _p(taps_y), ks_y, _p(scratch), _p(mean_std),
+                                        _p(out), _is_f32(out), _stream()), "clip_preprocess")
 
 
 # ------------------------------------------------------------------------------------------------ elementwise

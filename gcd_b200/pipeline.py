@@ -52,17 +52,67 @@ class GCDHotPath:
         return self
 
     @torch.no_grad()
-    def encode_cond_frames(self, frames, n_cond_frames=1, n_copies=1):
+    def encode_cond_frames(self, frames, n_cond_frames=1, n_copies=1, scale_factor=None):
         """VideoPredictionEmbedderWithEncoder.forward without noise augmentation (encoders/modules.py:1090-1109; the shipped
         configs set no sigma_sampler and n_cond_frames = n_copies = 1, infer_kubric.yaml:75-76): frames [B*T,3,H,W] in
         [-1,1] -> scale_factor * mode(encode), then "(b t) c h w -> b () (t c) h w" repeated n_copies times. The result is
-        the `concat` conditioning the UNet wrapper appends to the noisy latents (wrappers.py:24)."""
-        z = self.encoder.encode_mode(frames.to(self.device, non_blocking=True), self.quant[0], self.quant[1], self.scale_factor)
+        the `concat` conditioning the UNet wrapper appends to the noisy latents (wrappers.py:24). `scale_factor` defaults to
+        the first-stage scale of this pipeline."""
+        s = self.scale_factor if scale_factor is None else scale_factor
+        z = self.encoder.encode_mode(frames.to(self.device, non_blocking=True), self.quant[0], self.quant[1], s)
         if n_cond_frames == 1 and n_copies == 1:
             return z
         bt, c, h, w = z.shape
         z = z.view(bt // n_cond_frames, 1, n_cond_frames * c, h, w)
         return z.expand(-1, n_copies, -1, -1, -1).reshape(-1, n_cond_frames * c, h, w)
+
+    def load_clip(self, state, vit_cfg=None):
+        """The conditioner's OpenCLIP ViT-H/14 image tower (gcd_b200.embedders.FrozenOpenCLIPImageEmbedder). `state`: its state
+        dict, keys `model.visual.*` (the text-side leftovers of a checkpoint may be included). vit_cfg: a smaller tower."""
+        from .embedders import FrozenOpenCLIPImageEmbedder
+        clip = FrozenOpenCLIPImageEmbedder(vit_cfg=vit_cfg)
+        missing, unexpected = clip.load_state_dict(state, strict=False)
+        if missing or unexpected:
+            raise KeyError(f"load_clip: missing {list(missing)[:5]}, unexpected {list(unexpected)[:5]}")
+        self.clip = clip.to(self.device)
+        return self
+
+    def load_spherical(self, weight, bias):
+        """SphericalEmbedder.proj of the Kubric conditioner (infer_kubric.yaml:105-110): weight [128, 13], bias [128]."""
+        from .embedders import SphericalEmbedder
+        self.spherical = SphericalEmbedder(weight.shape[0])
+        self.spherical.proj.weight.data.copy_(weight)
+        self.spherical.proj.bias.data.copy_(bias)
+        self.spherical.to(self.device)
+        return self
+
+    @torch.no_grad()
+    def condition(self, batch, cond_scale_factor=1.0):
+        """(c, uc) of GeneralConditioner.get_unconditional_conditioning(batch, batch_uc=batch,
+        force_uc_zero_embeddings=["cond_frames", "cond_frames_without_noise"]) (encoders/modules.py:84-208,
+        models/diffusion.py:522-524) for the GCD embedder lists (infer_kubric.yaml:45-110, infer_pardom.yaml):
+            crossattn  FrozenOpenCLIPImagePredictionEmbedder(cond_frames_without_noise)   [BT, 1, 1024]   (load_clip)
+            vector     cat(fps_id, motion_bucket_id, cond_aug) timestep embeddings (256 each) [+ SphericalEmbedder(
+                       scaled_relative_angles), 128, when the UNet takes an aux embedding]          [BT, 768 | 896]
+            concat     VideoPredictionEmbedderWithEncoder(cond_frames)                  [BT, 4, H/8, W/8] (load_cond_encoder)
+        uc: crossattn and concat zero, vector equal to c's. `cond_scale_factor` is that embedder's scale_factor (the configs
+        leave the reference default 1.0). Noise augmentation of cond_frames is the caller's (eval_utils.py:224-225)."""
+        from .embedders import ConcatTimestepEmbedderND
+        dev = self.device
+        get = lambda k: batch[k].to(dev, non_blocking=True)
+        frames = get("cond_frames_without_noise")
+        ca = self.clip(frames)[:, None, :]                          # n_cond_frames = n_copies = 1: "(b t) d -> b t d"
+        ts = ConcatTimestepEmbedderND(256)
+        vec = [ts(get(k)) for k in ("fps_id", "motion_bucket_id", "cond_aug")]
+        if self.unet_cfg.get("aux_emb_dim", 0):
+            if getattr(self, "spherical", None) is None:
+                raise RuntimeError("condition: this UNet takes the spherical camera embedding; call load_spherical first")
+            vec.append(self.spherical(get("scaled_relative_angles")))
+        vector = torch.cat(vec, 1)
+        concat = self.encode_cond_frames(get("cond_frames"), scale_factor=cond_scale_factor)
+        c = {"crossattn": ca, "vector": vector, "concat": concat}
+        uc = {"crossattn": torch.zeros_like(ca), "vector": vector.clone(), "concat": torch.zeros_like(concat)}
+        return c, uc
 
     @torch.no_grad()
     def sample_latents(self, noise, c, uc, num_steps=None):

@@ -28,7 +28,7 @@ int64_t gcd_launch_count(void);
 
 /* Fused epilogue applied to every tensor-core op (rows r of the output, columns n):
  *   x      = acc[r,n] + bias[n] + rowvec[(r / rows_per_vec) * ld_rowvec + n]
- *   x      = act(x)                      (act: 0 none, 1 SiLU)
+ *   x      = act(x)                      (act: 0 none, 1 SiLU, 2 exact GELU 0.5 x (1 + erf(x / sqrt 2)) = nn.GELU())
  *   geglu: columns come in interleaved blocks of 16 value / 16 gate;  x = value * gelu_erf(gate)
  *          and the output has N/2 columns          (attention.py:87-94 GEGLU)
  *   out    = a_acc * x + a_res1 * res1[r,n] + a_res2 * res2[r,n]
@@ -100,6 +100,10 @@ int gcd_groupnorm_apply(const void* in, int in_f32, int64_t n_img, int64_t rows,
  * (video_attention.py:266-287 time_pos_embed) and the sum written to sum_out (float32) when non-NULL. */
 int gcd_layernorm(const float* in, int64_t rows, int C, const float* gamma, const float* beta, float eps,
                   const float* add, int64_t add_rows_per, int64_t add_mod, float* sum_out, void* out, void* stream);
+/* The same LayerNorm (with the same optional `add`) written as float32 [rows, C]: open_clip VisionTransformer's ln_pre, whose
+ * output is the residual stream of the tower. `out` must not alias `in`. */
+int gcd_layernorm_f32(const float* in, int64_t rows, int C, const float* gamma, const float* beta, float eps,
+                      const float* add, int64_t add_rows_per, int64_t add_mod, float* out, void* stream);
 
 /* ---- attention ------------------------------------------------------------------------------------------- */
 /* Spatial self-attention softmax(QK^T/sqrt(64))V, head_dim 64 (attention.py:255-344 CrossAttention with
@@ -109,6 +113,11 @@ int gcd_attention_spatial(const void* qkv, int frames, int tokens, int heads, vo
 /* Temporal self-attention over T frames per (clip, spatial position) (video_attention.py:109-140 attn1 after the
  * "(b t) s c -> (b s) t c" rearrange, done here by indexing). qkv/out laid out as above with frames = clips*T. */
 int gcd_attention_temporal(const void* qkv, int clips, int T, int tokens, int heads, void* out, void* stream);
+/* ViT self-attention with head_dim 80 (open_clip ViT-H/14 resblocks: nn.MultiheadAttention, 16 heads, 257 tokens):
+ * softmax(q k^T / sqrt(80)) v per (image, head) with fp32 softmax; scores are never written to memory.
+ * qkv: act [n, L, 3*heads*80] = in_proj output (q | k | v, head index outer within each third); out: act [n, L, heads*80].
+ * L in 1..1024. */
+int gcd_attention_d80(const void* qkv, int n, int L, int heads, void* out, void* stream);
 /* Row softmax of float32 scores [rows, cols] * scale -> act probs (model.py:161-201 AttnBlock, d=512 single head). */
 int gcd_softmax_rows(const float* in, int64_t rows, int cols, float scale, void* out, void* stream);
 
@@ -149,6 +158,17 @@ int gcd_timestep_embedding(const float* t, int n, int dim, float max_period, voi
 /* SphericalEmbedder.forward (encoders/modules.py:247-287; SURVEY.md 8(f) rank 1): x[n,3] = (azimuth, elevation, radius) float32
  * -> out[n,dim] float32 = [cos/sin of 1x,2x,4x azimuth | same for elevation | radius] * w[dim,13]^T + b[dim]. */
 int gcd_spherical_embed(const float* x, int n, const float* w, const float* b, int dim, float* out, void* stream);
+
+/* FrozenOpenCLIPImageEmbedder.preprocess (encoders/modules.py:703-715) + the ViT's conv1 patch unfold, fp32 arithmetic:
+ * kornia 0.7.0 resize(x, (224, 224), bicubic, align_corners=True, antialias) -> (x + 1) / 2 -> (x - mean[c]) / std[c].
+ * in: float32 NCHW [n, 3, H, W]. Antialias (when ks_x > 0): separable Gaussian blur, taps_x (ks_x, odd) along W first, then
+ * taps_y along H, 'reflect' border; taps are device float32 arrays computed by the host. Then PyTorch bicubic
+ * (A = -0.75, align_corners=True, clamped taps); a 224x224 input is used unchanged (no blur, no resize).
+ * scratch: float32 [2*n*3*H*W] when blurring, else unused. mean_std: device float32 {mean[3], std[3]}.
+ * out: [n*257, 640], act (out_f32 = 0) or float32 (1); row 0 of every image is zero (class-token slot), row
+ * 1 + py*16 + px holds the 14x14x3 patch at (py, px) ordered (ky, kx, c) in columns 0..587, columns 588..639 zero. */
+int gcd_clip_preprocess(const float* in, int n, int H, int W, const float* taps_x, int ks_x, const float* taps_y, int ks_y,
+                        float* scratch, const float* mean_std, void* out, int out_f32, void* stream);
 
 /* ---- sampler step (sampling.py:101-121, denoiser.py:23-49, guiders.py:79-100, wrappers.py:23-34) ------------ */
 /* The scalar coefficients c_in/c_out/c_skip (denoiser_scaling.py:53-61) and dt = sigma_next - sigma_hat are computed
