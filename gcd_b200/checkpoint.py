@@ -13,7 +13,7 @@ that module tree for the parts this package replaces, so the same call works and
     conditioner.embedders.<i>.*                  gcd_b200.embedders (optional, HotPathRoot(conditioner=...))
 
 Host-side plumbing only: no kernels involved; the modules repack their weights for the CUDA engines on the next forward
-(gcd_b200.unet.weights_key).
+(gcd_b200.engine.weights_key).
 """
 import os
 

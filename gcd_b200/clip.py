@@ -15,7 +15,7 @@ package's kernels: open_clip 2.23.0 `VisionTransformer.forward` after kornia 0.7
 import torch
 
 from . import ops
-from .unet import BufferPool
+from .engine import BufferPool
 
 VIT_H14 = dict(width=1280, layers=32, heads=16, patch=14, image=224, embed=1024)
 # Test-size tower with the same head width, patch and image size. Width 320: gcd_layernorm needs C % 64 == 0 and the attention

@@ -11,21 +11,12 @@ import torch
 import torch.nn as nn
 
 from . import clip, ops
-from .unet import register_param_tree, weights_key
+from .engine import EngineCache, need_option, reference_base, register_param_tree
 
-
-def _reference_base():
-    """The reference GeneralConditioner asserts `isinstance(embedder, AbstractEmbModel)` (encoders/modules.py:93-96): when
-    `sgm` imports, derive from its AbstractEmbModel so a YAML `target:` swap passes that gate; standalone, a plain nn.Module
-    carrying the same three attributes (encoders/modules.py:40-81)."""
-    try:
-        from sgm.modules.encoders.modules import AbstractEmbModel as Ref   # noqa: WPS433
-        return Ref
-    except Exception:
-        return nn.Module
-
-
-_RefBase = _reference_base()
+# The reference GeneralConditioner asserts `isinstance(embedder, AbstractEmbModel)` (encoders/modules.py:93-96): when `sgm`
+# imports, the embedders derive from its AbstractEmbModel so a YAML `target:` swap passes that gate; standalone, from a plain
+# nn.Module carrying the same three attributes (encoders/modules.py:40-81).
+_RefBase = reference_base("sgm.modules.encoders.modules", "AbstractEmbModel")
 
 
 class _EmbBase(_RefBase):
@@ -91,11 +82,7 @@ class FrozenOpenCLIPImageEmbedder(_EmbBase):
                  ucg_rate=0.0, unsqueeze_dim=False, repeat_to_max_len=False, num_image_crops=0, output_tokens=False,
                  init_device=None, vit_cfg=None):
         super().__init__()
-
-        def need(cond, what):
-            if not cond:
-                raise NotImplementedError(f"gcd_b200.FrozenOpenCLIPImageEmbedder: {what} is not built (GCD sets none of these)")
-
+        need = need_option("FrozenOpenCLIPImageEmbedder")
         need(arch == "ViT-H-14", f"arch={arch!r}")
         need(num_image_crops == 0, "num_image_crops > 0")
         need(not output_tokens, "output_tokens=True")
@@ -114,15 +101,11 @@ class FrozenOpenCLIPImageEmbedder(_EmbBase):
         if freeze:
             for p in self.parameters():
                 p.requires_grad = False
-        self._engine, self._engine_key = None, None
+        self._engines = EngineCache()
 
     def engine(self, device):
-        key = weights_key(self.model.visual, device)
-        if self._engine is None or self._engine_key != key:
-            self._engine = None
-            self._engine = clip.ClipEngine(self.vit_cfg, self.model.visual.state_dict(), device)
-            self._engine_key = key
-        return self._engine
+        visual = self.model.visual
+        return self._engines.get(visual, device, lambda: clip.ClipEngine(self.vit_cfg, visual.state_dict(), device))
 
     @torch.no_grad()
     def forward(self, image, no_dropout=False):

@@ -204,11 +204,6 @@ def conv_t3(x, w, ep):
 
 
 # ------------------------------------------------------------------------------------------------ norms
-def zero_stats(stats, n_img, groups=32):
-    with _timed("elem", 0.0, n_img * groups * 2 * 8):
-        check(lib().gcd_memset_async(_p(stats), 0, n_img * groups * 2 * 8, _stream()), "memset")
-
-
 def zero_tensor(t):
     """One memset over a whole (contiguous) workspace tensor."""
     nbytes = t.numel() * t.element_size()

@@ -14,102 +14,13 @@ Exact algebraic shortcuts taken (SURVEY.md §8(a) facts 1-5, all parity-tested a
   - all 50 `emb_layers` Linear(SiLU(emb)) run as one GEMM per forward;
   - image_only_indicator is all zeros => AlphaBlender alpha = sigmoid(mix_factor) (scalar per blender).
 """
-import math
 import os
 
 import torch
 import torch.nn as nn
 
 from . import ops, spec
-
-
-# ----------------------------------------------------------------------------------------------------------------------
-class _Node(nn.Module):
-    """Anonymous container used to reproduce the reference module tree (and therefore its state_dict keys)."""
-
-
-def register_param_tree(root, shapes, init=None):
-    """Registers nn.Parameters under nested _Node modules so that root.state_dict() has exactly the keys of `shapes`."""
-    for key, shape in shapes.items():
-        parts = key.split(".")
-        mod = root
-        for p in parts[:-1]:
-            if not hasattr(mod, p):
-                mod.add_module(p, _Node())
-            mod = getattr(mod, p)
-        t = torch.zeros(shape) if init is None else init(key, shape)
-        # requires_grad=True like any nn.Module parameter: the reference's LitEma (modules/ema.py) only shadows parameters
-        # with requires_grad, and DiffusionEngine.ema_scope swaps them in with `param.data.copy_` — see weights_key()
-        mod.register_parameter(parts[-1], nn.Parameter(t, requires_grad=True))
-
-
-def weights_key(module, device):
-    """Cache key of a drop-in module's packed engine: (data_ptr, _version) of every parameter PLUS a content probe of nine
-    tensors spread over the parameter list. `_version` alone misses `param.data.copy_(...)` — exactly what the reference's
-    LitEma.copy_to / restore do (modules/ema.py) — so an EMA swap would otherwise keep running the stale packed weights.
-    Costs one small device->host read per engine() call (once per sample on the fused path)."""
-    ps = list(module.parameters())
-    meta = tuple((p.data_ptr(), p._version) for p in ps)
-    probe = ps[::max(1, len(ps) // 8)][:8] + [ps[-1]]
-    vals = torch.stack([p.detach().reshape(-1)[:512].double().sum().cpu() for p in probe]).tolist()
-    return (str(device), meta, tuple(vals))
-
-
-FUSE_CONCAT_STATS = True      # skip-concat kernel also produces the following GroupNorm's statistics
-
-
-class BufferPool:
-    """Named device workspaces, allocated once per (name, shape, dtype) and reused across blocks and steps."""
-
-    def __init__(self, device):
-        self.device = device
-        self.bufs = {}
-
-    def get(self, name, shape, dtype):
-        key = (name, tuple(shape), dtype)
-        b = self.bufs.get(key)
-        if b is None:
-            b = torch.empty(shape, device=self.device, dtype=dtype)
-            self.bufs[key] = b
-        return b
-
-    def nbytes(self):
-        return sum(b.numel() * b.element_size() for b in self.bufs.values())
-
-    def release(self, name):
-        """Drops the workspaces named `name` (their memory returns to the caching allocator)."""
-        self.bufs = {k: b for k, b in self.bufs.items() if k[0] != name}
-
-    def release_rows(self, rows):
-        """Drops the workspaces whose leading dimension is `rows` (their memory returns to the caching allocator)."""
-        self.bufs = {k: b for k, b in self.bufs.items() if k[1][:1] != (rows,)}
-
-
-class StatsArena:
-    """float64 scratch for the GroupNorm statistics that tensor-core epilogues accumulate (gcd_epilogue.gn_stats): one slot per
-    producer -> consumer hand-off of a forward pass, the WHOLE arena zeroed by one memset at the start of the pass (round 1
-    zeroed a ring buffer before each of the ~130 producers: ~130 extra launches per CFG forward, 2 % of its time in the `elem`
-    class of tools/prof_forward.py)."""
-    SLOTS = 256
-
-    def __init__(self, pool):
-        self.pool, self.slot, self.buf, self.i = pool, 0, None, 0
-
-    def reset(self, n_img):
-        """n_img: the largest number of images (frames) any statistics of this pass are kept for."""
-        need = max(n_img, 64) * 64
-        if need > self.slot:
-            self.slot = need
-            self.buf = self.pool.get("gn_arena", (self.SLOTS * need,), torch.float64)
-        self.i = 0
-        ops.zero_tensor(self.buf)
-
-    def take(self, n_img):
-        need = max(n_img, 64) * 64
-        assert need <= self.slot and self.i < self.SLOTS, "GroupNorm statistics arena exhausted"
-        st = self.buf[self.i * self.slot:(self.i + 1) * self.slot]
-        self.i += 1
-        return st
+from .engine import Engine, EngineCache, need_option, register_param_tree
 
 
 def _geglu_interleave(w, b):
@@ -120,89 +31,59 @@ def _geglu_interleave(w, b):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-class UNetEngine:
-    def __init__(self, cfg, state, device, T_pack=None):
+class UNetEngine(Engine):
+    def __init__(self, cfg, state, device):
         """state: mapping reference-key -> float32 tensor (any device)."""
+        super().__init__(device)
         self.cfg = cfg
-        self.device = torch.device(device)
-        self.AD = ops.act_dtype()
-        self.pool = BufferPool(self.device)
         self.plan = spec.unet_plan(cfg)
-        self.w = {}
         self._pe_cache = {}
         self.debug = None          # set to a list to record every layer's output (tools/bisect_batch.py)
-        self.arena = StatsArena(self.pool)
         self.use_graphs = os.environ.get("GCD_NO_GRAPH", "0") != "1"
         self._graphs = {}
         self._pack(state)
 
     # ------------------------------------------------------------------------------------------------ weight packing
     def _pack(self, sd):
-        dev, AD = self.device, self.AD
-        g = lambda k: sd[k].detach().to(dev, torch.float32)
-        W = self.w
-
-        def lin(name, key):
-            W[name + ".w"] = g(key + ".weight").to(AD).contiguous()
-            if (key + ".bias") in sd:
-                W[name + ".b"] = g(key + ".bias").contiguous()
-
-        def conv3(name, key, cin_pad=None):
-            w = g(key + ".weight")                                   # [Co, Ci, 3, 3]
-            if cin_pad is not None and cin_pad != w.shape[1]:
-                w = torch.cat([w, w.new_zeros(w.shape[0], cin_pad - w.shape[1], 3, 3)], 1)
-            W[name + ".w"] = w.permute(0, 2, 3, 1).reshape(w.shape[0], -1).to(AD).contiguous()
-            W[name + ".b"] = g(key + ".bias").contiguous()
-
-        def convt(name, key):
-            w = g(key + ".weight")[:, :, :, 0, 0]                    # [Co, Ci, 3]
-            W[name + ".w"] = w.permute(0, 2, 1).reshape(w.shape[0], -1).to(AD).contiguous()
-            W[name + ".b"] = g(key + ".bias").contiguous()
-
-        def norm(name, key):
-            W[name + ".g"] = g(key + ".weight").contiguous()
-            W[name + ".b"] = g(key + ".bias").contiguous()
-
-        def geglu(name, key):
-            w, b = _geglu_interleave(g(key + ".weight"), g(key + ".bias"))
-            W[name + ".w"], W[name + ".b"] = w.to(AD).contiguous(), b
+        g = lambda k: self._f32(sd[k])
 
         def attn(p):
-            W[p + ".qkv.w"] = torch.cat([g(p + ".attn1.to_q.weight"), g(p + ".attn1.to_k.weight"),
-                                         g(p + ".attn1.to_v.weight")], 0).to(AD).contiguous()
-            lin(p + ".attn1.out", p + ".attn1.to_out.0")
-            lin(p + ".attn2.v", p + ".attn2.to_v")
-            lin(p + ".attn2.out", p + ".attn2.to_out.0")
+            qkv = [g(p + ".attn1.to_q.weight"), g(p + ".attn1.to_k.weight"), g(p + ".attn1.to_v.weight")]
+            self._lin(sd, p + ".qkv", (torch.cat(qkv, 0), None))     # the fp32 concatenation is freed right after packing
+            self._lin(sd, p + ".attn1.out", p + ".attn1.to_out.0")
+            self._lin(sd, p + ".attn2.v", p + ".attn2.to_v")
+            self._lin(sd, p + ".attn2.out", p + ".attn2.to_out.0")
+
+        def geglu(name, key):
+            self._lin(sd, name, _geglu_interleave(g(key + ".weight"), g(key + ".bias")))
 
         for k in ("time_embed.0", "time_embed.2", "label_emb.0.0", "label_emb.0.2"):
-            lin(k, k)
+            self._lin(sd, k, k)
         if self.cfg["aux_emb_dim"] > 0:
-            lin("aux_label_emb.0", "aux_label_emb.0")
-            lin("aux_label_emb.2", "aux_label_emb.2")
+            self._lin(sd, "aux_label_emb.0", "aux_label_emb.0")
+            self._lin(sd, "aux_label_emb.2", "aux_label_emb.2")
         inp, mid, out = self.plan
         emb_w, emb_b, self.emb_off, off = [], [], {}, 0
-        self.alpha = {}
         for layers in inp + [mid] + out:
             for kind, p, cin, cout in layers:
                 if kind == "conv_in":
-                    conv3(p, p, cin_pad=64)
+                    self._conv3(sd, p, p, cin_pad=64)
                 elif kind == "down":
-                    conv3(p, p + ".op")
+                    self._conv3(sd, p, p + ".op")
                 elif kind == "up":
-                    conv3(p, p + ".conv")
+                    self._conv3(sd, p, p + ".conv")
                 elif kind == "vrb":
-                    norm(p + ".n1", p + ".in_layers.0")
-                    conv3(p + ".c1", p + ".in_layers.2")
-                    norm(p + ".n2", p + ".out_layers.0")
-                    conv3(p + ".c2", p + ".out_layers.3")
+                    self._norm(sd, p + ".n1", p + ".in_layers.0")
+                    self._conv3(sd, p + ".c1", p + ".in_layers.2")
+                    self._norm(sd, p + ".n2", p + ".out_layers.0")
+                    self._conv3(sd, p + ".c2", p + ".out_layers.3")
                     if cin != cout:
-                        W[p + ".skip.w"] = g(p + ".skip_connection.weight")[:, :, 0, 0].to(AD).contiguous()
-                        W[p + ".skip.b"] = g(p + ".skip_connection.bias").contiguous()
+                        self._lin(sd, p + ".skip", p + ".skip_connection")
                     q = p + ".time_stack"
-                    norm(q + ".n1", q + ".in_layers.0")
-                    convt(q + ".c1", q + ".in_layers.2")
-                    norm(q + ".n2", q + ".out_layers.0")
-                    convt(q + ".c2", q + ".out_layers.3")
+                    self._norm(sd, q + ".n1", q + ".in_layers.0")
+                    self._convt(sd, q + ".c1", q + ".in_layers.2")
+                    self._norm(sd, q + ".n2", q + ".out_layers.0")
+                    self._convt(sd, q + ".c2", q + ".out_layers.3")
                     for e in (p, q):
                         emb_w.append(g(e + ".emb_layers.1.weight"))
                         emb_b.append(g(e + ".emb_layers.1.bias"))
@@ -210,41 +91,28 @@ class UNetEngine:
                         off += cout
                     self.alpha[p] = float(torch.sigmoid(g(p + ".time_mixer.mix_factor")).item())
                 elif kind == "svt":
-                    norm(p + ".norm", p + ".norm")
-                    lin(p + ".proj_in", p + ".proj_in")
-                    lin(p + ".proj_out", p + ".proj_out")
+                    self._norm(sd, p + ".norm", p + ".norm")
+                    self._lin(sd, p + ".proj_in", p + ".proj_in")
+                    self._lin(sd, p + ".proj_out", p + ".proj_out")
                     assert self.cfg["transformer_depth"] == 1, "transformer_depth != 1 is not used by GCD"
                     s, t = p + ".transformer_blocks.0", p + ".time_stack.0"
                     for blk in (s, t):
                         attn(blk)
                         for n in ("norm1", "norm3") + (("norm_in",) if blk == t else ()):
-                            norm(blk + "." + n, blk + "." + n)
+                            self._norm(sd, blk + "." + n, blk + "." + n)
                         geglu(blk + ".ff.0", blk + ".ff.net.0.proj")
-                        lin(blk + ".ff.2", blk + ".ff.net.2")
+                        self._lin(sd, blk + ".ff.2", blk + ".ff.net.2")
                     geglu(t + ".ff_in.0", t + ".ff_in.net.0.proj")
-                    lin(t + ".ff_in.2", t + ".ff_in.net.2")
-                    lin(p + ".tpe.0", p + ".time_pos_embed.0")
-                    lin(p + ".tpe.2", p + ".time_pos_embed.2")
+                    self._lin(sd, t + ".ff_in.2", t + ".ff_in.net.2")
+                    self._lin(sd, p + ".tpe.0", p + ".time_pos_embed.0")
+                    self._lin(sd, p + ".tpe.2", p + ".time_pos_embed.2")
                     self.alpha[p] = float(torch.sigmoid(g(p + ".time_mixer.mix_factor")).item())
-        W["emb_all.w"] = torch.cat(emb_w, 0).to(AD).contiguous()
-        W["emb_all.b"] = torch.cat(emb_b, 0).contiguous()
+        self._lin(sd, "emb_all", (torch.cat(emb_w, 0), torch.cat(emb_b, 0)))
         self.emb_total = off
-        norm("out.0", "out.0")
-        conv3("out.2", "out.2")
-        self.weight_bytes = sum(t.numel() * t.element_size() for t in W.values())
+        self._norm(sd, "out.0", "out.0")
+        self._conv3(sd, "out.2", "out.2")
 
     # ------------------------------------------------------------------------------------------------ small helpers
-    def _gn(self, x, n_img, rows, C, name, eps, silu, out, stats=None):
-        """GroupNorm(32) (+SiLU) -> act. `stats`: statistics already accumulated by the producing tensor-core op."""
-        st = stats if stats is not None else self.pool.get("gn_stats", (max(n_img, 64) * 64,), torch.float64)
-        ops.groupnorm(x, n_img, rows, C, self.w[name + ".g"], self.w[name + ".b"], eps, silu, out, st,
-                      have_stats=stats is not None)
-
-    def _stats_req(self, n_img, C, rows_per_img):
-        """Zeroed float64 statistics slot (StatsArena, zeroed once per forward) + the epilogue descriptor."""
-        st = self.arena.take(n_img)
-        return st, (st, C // 32, 32, rows_per_img)
-
     def _mlp_small(self, x_act, k0, k2, out_f32, accumulate):
         """Linear -> SiLU -> Linear on a handful of rows (time_embed / label_emb / time_pos_embed)."""
         W = self.w
@@ -509,18 +377,12 @@ class UNetEngine:
             # The consumer is a ResBlock with cin != cout (1x1 skip conv): nothing reads the concat in fp32, so it is written in
             # the 16-bit operand type only (10 instead of 20 bytes per element over concat + GroupNorm + cast).
             first = layers[0]
-            cst = None
-            if FUSE_CONCAT_STATS and first[0] == "vrb" and first[2] != first[3]:
+            if first[0] == "vrb" and first[2] != first[3]:
                 cat = pool.get(f"cat16_{bi}", (n * hH * hW, hC + sC), AD)
-                cst, _ = self._stats_req(n, hC + sC, hH * hW)
-                ops.concat_channels(h, s, cat, stats=cst, n_img=n)
-            elif FUSE_CONCAT_STATS:
-                cat = pool.get(f"cat{bi}", (n * hH * hW, hC + sC), torch.float32)
-                cst, _ = self._stats_req(n, hC + sC, hH * hW)
-                ops.concat_channels(h, s, cat, stats=cst, n_img=n)
             else:
                 cat = pool.get(f"cat{bi}", (n * hH * hW, hC + sC), torch.float32)
-                ops.concat_channels(h, s, cat)
+            cst, _ = self._stats_req(n, hC + sC, hH * hW)
+            ops.concat_channels(h, s, cat, stats=cst, n_img=n)
             h, hH, hW, hC, hst = run(layers, cat, hH, hW, hC + sC, bi, "out", cst)
         rows = n * hH * hW
         a = pool.get(f"act_a{hC}", (rows, hC), AD)
@@ -547,11 +409,7 @@ class VideoUNet(nn.Module):
                  use_linear_in_transformer=False, adm_in_channels=None, aux_emb_dim=0, aux_zero_init=False,
                  disable_temporal_crossattention=False, max_ddpm_temb_period=10000):
         super().__init__()
-
-        def need(cond, what):
-            if not cond:
-                raise NotImplementedError(f"gcd_b200.VideoUNet: unsupported option ({what}); only the GCD configs are built")
-
+        need = need_option("VideoUNet")
         need(dims == 2 and conv_resample and not resblock_updown and not use_scale_shift_norm, "dims/resample/updown")
         need(num_classes == "sequential" and adm_in_channels is not None, "num_classes must be 'sequential'")
         need(num_head_channels == 64, "num_head_channels must be 64")
@@ -569,21 +427,14 @@ class VideoUNet(nn.Module):
         self.in_channels, self.model_channels, self.out_channels = in_channels, model_channels, out_channels
         self.adm_in_channels, self.aux_emb_dim, self.num_classes = adm_in_channels, aux_emb_dim, num_classes
         register_param_tree(self, spec.unet_param_shapes(self.cfg))
-        self._engine = None
-        self._engine_key = None
+        self._engines = EngineCache()
 
-    # weights may be (re)loaded at any time (init_from_ckpt, EMA swap through `.data.copy_`): repack lazily when any
-    # parameter changed (weights_key); `invalidate()` forces it for in-place edits the key cannot see
     def invalidate(self):
-        self._engine, self._engine_key = None, None
+        """Forces a repack at the next forward, for in-place weight edits that weights_key cannot see."""
+        self._engines.clear()
 
     def engine(self, device):
-        key = weights_key(self, device)
-        if self._engine is None or self._engine_key != key:
-            self._engine = None                                   # release the old packed weights / workspaces first
-            self._engine = UNetEngine(self.cfg, self.state_dict(), device)
-            self._engine_key = key
-        return self._engine
+        return self._engines.get(self, device, lambda: UNetEngine(self.cfg, self.state_dict(), device))
 
     @torch.no_grad()
     def forward(self, x, timesteps, context=None, y=None, time_context=None, num_video_frames=None,

@@ -14,86 +14,33 @@ import torch
 import torch.nn as nn
 
 from . import ops, spec
-from .unet import BufferPool, StatsArena, register_param_tree, weights_key
+from .engine import Engine, EngineCache, need_option, reference_base, register_param_tree
 
 
-class DecoderEngine:
-    def __init__(self, cfg, state, device):
-        self.cfg, self.device, self.AD = cfg, torch.device(device), ops.act_dtype()
-        self.pool = BufferPool(self.device)
-        self.plan = spec.decoder_plan(cfg)
-        self.w, self.alpha = {}, {}
-        self._pack(state)
+class _VAEEngine(Engine):
+    """What the VAE encoder and decoder share: channels-last fp32 residual stream, 16-bit tensor-core operands, the spatial
+    ResnetBlock and the mid AttnBlock."""
 
-    def _pack(self, sd):
-        dev, AD, W = self.device, self.AD, self.w
-        g = lambda k: sd[k].detach().to(dev, torch.float32)
+    def __init__(self, cfg, plan, device):
+        super().__init__(device)
+        self.cfg, self.plan = cfg, plan
 
-        def conv3(name, key, cin_pad=None):
-            w = g(key + ".weight")
-            if cin_pad is not None and cin_pad != w.shape[1]:
-                w = torch.cat([w, w.new_zeros(w.shape[0], cin_pad - w.shape[1], 3, 3)], 1)
-            W[name + ".w"] = w.permute(0, 2, 3, 1).reshape(w.shape[0], -1).to(AD).contiguous()
-            W[name + ".b"] = g(key + ".bias").contiguous()
+    def _pack_res(self, sd, p, cin, cout):
+        self._norm(sd, p + ".n1", p + ".norm1")
+        self._conv3(sd, p + ".c1", p + ".conv1")
+        self._norm(sd, p + ".n2", p + ".norm2")
+        self._conv3(sd, p + ".c2", p + ".conv2")
+        if cin != cout:
+            self._lin(sd, p + ".skip", p + ".nin_shortcut")
 
-        def convt(name, key):
-            w = g(key + ".weight")[:, :, :, 0, 0]
-            W[name + ".w"] = w.permute(0, 2, 1).reshape(w.shape[0], -1).to(AD).contiguous()
-            W[name + ".b"] = g(key + ".bias").contiguous()
+    def _pack_attn(self, sd, p):
+        self._norm(sd, p + ".norm", p + ".norm")
+        for n in ("q", "k", "v", "proj_out"):
+            self._lin(sd, f"{p}.{n}", f"{p}.{n}")
 
-        def conv1(name, key):
-            W[name + ".w"] = g(key + ".weight")[:, :, 0, 0].to(AD).contiguous()
-            W[name + ".b"] = g(key + ".bias").contiguous()
-
-        def norm(name, key):
-            W[name + ".g"], W[name + ".b"] = g(key + ".weight").contiguous(), g(key + ".bias").contiguous()
-
-        for kind, p, cin, cout in self.plan:
-            if kind == "conv_in":
-                conv3(p, p, cin_pad=64)
-            elif kind == "res":
-                norm(p + ".n1", p + ".norm1"); conv3(p + ".c1", p + ".conv1")
-                norm(p + ".n2", p + ".norm2"); conv3(p + ".c2", p + ".conv2")
-                if cin != cout:
-                    conv1(p + ".skip", p + ".nin_shortcut")
-                q = p + ".time_stack"
-                norm(q + ".n1", q + ".in_layers.0"); convt(q + ".c1", q + ".in_layers.2")
-                norm(q + ".n2", q + ".out_layers.0"); convt(q + ".c2", q + ".out_layers.3")
-                self.alpha[p] = float(torch.sigmoid(g(p + ".mix_factor")).item())
-            elif kind == "attn":
-                norm(p + ".norm", p + ".norm")
-                for n in ("q", "k", "v", "proj_out"):
-                    conv1(f"{p}.{n}", f"{p}.{n}")
-            elif kind == "up":
-                conv3(p, p + ".conv")
-            elif kind == "out":
-                norm("norm_out", "norm_out")
-                conv3("conv_out", "conv_out")
-                W["tmix.w"] = g("conv_out.time_mix_conv.weight").reshape(-1).contiguous()   # [co, ci, kt, 1, 1]
-                W["tmix.b"] = g("conv_out.time_mix_conv.bias").contiguous()
-        self.weight_bytes = sum(t.numel() * t.element_size() for t in W.values())
-
-    def _gn(self, x, n_img, rows, C, name, eps, silu, out, stats=None):
-        st = stats if stats is not None else self.pool.get("gn_stats", (max(n_img, 64) * 64,), torch.float64)
-        ops.groupnorm(x, n_img, rows, C, self.w[name + ".g"], self.w[name + ".b"], eps, silu, out, st,
-                      have_stats=stats is not None)
-
-    def _stats_req(self, n_img, C, rows_per_img):
-        """Zeroed statistics slot for the GroupNorm that consumes the tensor a conv is about to write (fused in its epilogue);
-        the arena is zeroed once per forward."""
-        if getattr(self, "arena", None) is None:
-            self.arena = StatsArena(self.pool)
-        st = self.arena.take(n_img)
-        return st, (st, C // 32, 32, rows_per_img)
-
-    def _arena_reset(self, n_img):
-        if getattr(self, "arena", None) is None:
-            self.arena = StatsArena(self.pool)
-        self.arena.reset(n_img)
-
-    def _res(self, p, x, cin, cout, n, B, T, H, Wd, tag, x_stats=None):
-        """temporal_ae.VideoResBlock.forward (temporal_ae.py:64-83) over ResnetBlock.forward (model.py:127-151).
-        Returns (x_out, per-frame GroupNorm statistics of x_out or None)."""
+    def _res2d(self, p, x, cin, cout, n, H, Wd, tag, out_geom, x_stats=None):
+        """ResnetBlock.forward with temb=None (model.py:127-151). `out_geom`: (images, rows per image) of the GroupNorm that
+        consumes the output, whose statistics conv2 accumulates. Returns (x_out fp32, those statistics or None)."""
         W, pool, AD = self.w, self.pool, self.AD
         HW, rows = H * Wd, n * H * Wd
         a = pool.get(f"a{cin}_{rows}", (rows, cin), AD)
@@ -111,17 +58,8 @@ class DecoderEngine:
             res = xs
         else:
             res = x
-        st, req = self._stats_req(B, cout, T * HW)
+        st, req = self._stats_req(out_geom[0], cout, out_geom[1])
         ok = ops.conv2d_3x3(a2.view(n, H, Wd, cout), W[p + ".c2.w"], ops.make_ep(xs, bias=W[p + ".c2.b"], res1=res, gn_stats=req))
-        q = p + ".time_stack"
-        self._gn(xs, B, T * HW, cout, q + ".n1", 1e-5, True, a2, stats=st if ok else None)
-        st, req = self._stats_req(B, cout, T * HW)
-        ok = ops.conv_t3(a2.view(B, T, HW, cout), W[q + ".c1.w"], ops.make_ep(h1, bias=W[q + ".c1.b"], gn_stats=req))
-        self._gn(h1, B, T * HW, cout, q + ".n2", 1e-5, True, a2, stats=st if ok else None)
-        # x = alpha * (x_s + conv) + (1 - alpha) * x_s = x_s + alpha * conv     (temporal_ae.py:79-80)
-        st, req = self._stats_req(n, cout, HW)
-        ok = ops.conv_t3(a2.view(B, T, HW, cout), W[q + ".c2.w"],
-                         ops.make_ep(xs, bias=W[q + ".c2.b"], a_acc=self.alpha[p], res1=xs, gn_stats=req))
         return xs, (st if ok else None)
 
     def _attn(self, p, x, C, n, S, x_stats=None):
@@ -151,12 +89,58 @@ class DecoderEngine:
         ops.linear(o, W[p + ".proj_out.w"], ops.make_ep(x, bias=W[p + ".proj_out.b"], res1=x))
         return x
 
+
+class DecoderEngine(_VAEEngine):
+    def __init__(self, cfg, state, device):
+        super().__init__(cfg, spec.decoder_plan(cfg), device)
+        self._pack(state)
+
+    def _pack(self, sd):
+        for kind, p, cin, cout in self.plan:
+            if kind == "conv_in":
+                self._conv3(sd, p, p, cin_pad=64)
+            elif kind == "res":
+                self._pack_res(sd, p, cin, cout)
+                q = p + ".time_stack"
+                self._norm(sd, q + ".n1", q + ".in_layers.0")
+                self._convt(sd, q + ".c1", q + ".in_layers.2")
+                self._norm(sd, q + ".n2", q + ".out_layers.0")
+                self._convt(sd, q + ".c2", q + ".out_layers.3")
+                self.alpha[p] = float(torch.sigmoid(self._f32(sd[p + ".mix_factor"])).item())
+            elif kind == "attn":
+                self._pack_attn(sd, p)
+            elif kind == "up":
+                self._conv3(sd, p, p + ".conv")
+            elif kind == "out":
+                self._norm(sd, "norm_out", "norm_out")
+                self._conv3(sd, "conv_out", "conv_out")
+                self.w["tmix.w"] = self._f32(sd["conv_out.time_mix_conv.weight"]).reshape(-1).contiguous()   # [co, ci, kt, 1, 1]
+                self.w["tmix.b"] = self._f32(sd["conv_out.time_mix_conv.bias"]).contiguous()
+
+    def _res(self, p, x, cin, cout, n, B, T, H, Wd, tag, x_stats=None):
+        """temporal_ae.VideoResBlock.forward (temporal_ae.py:64-83) over ResnetBlock.forward (model.py:127-151).
+        Returns (x_out, per-frame GroupNorm statistics of x_out or None)."""
+        W, pool, AD = self.w, self.pool, self.AD
+        HW, rows = H * Wd, n * H * Wd
+        xs, st = self._res2d(p, x, cin, cout, n, H, Wd, tag, (B, T * HW), x_stats=x_stats)
+        h1, a2 = pool.get(f"h{cout}_{rows}", (rows, cout), AD), pool.get(f"a{cout}_{rows}", (rows, cout), AD)
+        q = p + ".time_stack"
+        self._gn(xs, B, T * HW, cout, q + ".n1", 1e-5, True, a2, stats=st)
+        st, req = self._stats_req(B, cout, T * HW)
+        ok = ops.conv_t3(a2.view(B, T, HW, cout), W[q + ".c1.w"], ops.make_ep(h1, bias=W[q + ".c1.b"], gn_stats=req))
+        self._gn(h1, B, T * HW, cout, q + ".n2", 1e-5, True, a2, stats=st if ok else None)
+        # x = alpha * (x_s + conv) + (1 - alpha) * x_s = x_s + alpha * conv     (temporal_ae.py:79-80)
+        st, req = self._stats_req(n, cout, HW)
+        ok = ops.conv_t3(a2.view(B, T, HW, cout), W[q + ".c2.w"],
+                         ops.make_ep(xs, bias=W[q + ".c2.b"], a_acc=self.alpha[p], res1=xs, gn_stats=req))
+        return xs, (st if ok else None)
+
     def forward_cl(self, z_cl, n, H, Wd, T, out_nchw):
         """z_cl: act channels-last [n, H, W, 64]; writes float32 NCHW [n, out_ch, 8H, 8W] into out_nchw."""
         W, pool, AD = self.w, self.pool, self.AD
         assert n % T == 0
         B = n // T
-        self._arena_reset(n)
+        self.arena.reset(n)
         h, hH, hW, hC, hst = None, H, Wd, None, None
         for i, (kind, p, cin, cout) in enumerate(self.plan):
             rows = n * hH * hW
@@ -194,7 +178,7 @@ class DecoderEngine:
         return out_nchw
 
 
-class EncoderEngine(DecoderEngine):
+class EncoderEngine(_VAEEngine):
     """VAE Encoder of the conditioning frames (diffusionmodules/model.py:487-601; SURVEY.md §8(f) rank 1): the same
     channels-last fp32-residual design and the same kernels as the decoder, plus the stride-2 (0,1,0,1)-padded Downsample conv.
 
@@ -204,81 +188,35 @@ class EncoderEngine(DecoderEngine):
     """
 
     def __init__(self, cfg, state, device, post=None):
-        self.cfg, self.device, self.AD = cfg, torch.device(device), ops.act_dtype()
-        self.pool = BufferPool(self.device)
-        self.plan = spec.encoder_plan(cfg)
-        self.w, self.alpha = {}, {}
-        self._pack_encoder(state, post)
+        super().__init__(cfg, spec.encoder_plan(cfg), device)
+        self._pack(state, post)
 
-    def _pack_encoder(self, sd, post):
-        dev, AD, W = self.device, self.AD, self.w
-        g = lambda k: sd[k].detach().to(dev, torch.float32)
-
-        def conv3(name, w, b, cin_pad=None):
-            if cin_pad is not None and cin_pad != w.shape[1]:
-                w = torch.cat([w, w.new_zeros(w.shape[0], cin_pad - w.shape[1], 3, 3)], 1)
-            W[name + ".w"] = w.permute(0, 2, 3, 1).reshape(w.shape[0], -1).to(AD).contiguous()
-            W[name + ".b"] = b.contiguous()
-
-        def norm(name, key):
-            W[name + ".g"], W[name + ".b"] = g(key + ".weight").contiguous(), g(key + ".bias").contiguous()
-
+    def _pack(self, sd, post):
         for kind, p, cin, cout in self.plan:
             if kind == "conv_in":
-                conv3(p, g(p + ".weight"), g(p + ".bias"), cin_pad=64)
+                self._conv3(sd, p, p, cin_pad=64)
             elif kind == "res":
-                norm(p + ".n1", p + ".norm1"); conv3(p + ".c1", g(p + ".conv1.weight"), g(p + ".conv1.bias"))
-                norm(p + ".n2", p + ".norm2"); conv3(p + ".c2", g(p + ".conv2.weight"), g(p + ".conv2.bias"))
-                if cin != cout:
-                    W[p + ".skip.w"] = g(p + ".nin_shortcut.weight")[:, :, 0, 0].to(AD).contiguous()
-                    W[p + ".skip.b"] = g(p + ".nin_shortcut.bias").contiguous()
+                self._pack_res(sd, p, cin, cout)
             elif kind == "attn":
-                norm(p + ".norm", p + ".norm")
-                for n in ("q", "k", "v", "proj_out"):
-                    W[f"{p}.{n}.w"] = g(f"{p}.{n}.weight")[:, :, 0, 0].to(AD).contiguous()
-                    W[f"{p}.{n}.b"] = g(f"{p}.{n}.bias").contiguous()
+                self._pack_attn(sd, p)
             elif kind == "down":
-                conv3(p, g(p + ".conv.weight"), g(p + ".conv.bias"))
+                self._conv3(sd, p, p + ".conv")
             elif kind == "out":
-                norm("norm_out", "norm_out")
-                w, b = g("conv_out.weight"), g("conv_out.bias")
+                self._norm(sd, "norm_out", "norm_out")
+                w, b = self._f32(sd["conv_out.weight"]), self._f32(sd["conv_out.bias"])
                 if post is not None:
                     wq, bq, scale = post
-                    wq, bq = wq.detach().to(dev, torch.float32).reshape(wq.shape[0], -1), bq.detach().to(dev, torch.float32)
+                    wq, bq = self._f32(wq).reshape(wq.shape[0], -1), self._f32(bq)
                     w = float(scale) * torch.einsum("oc,cikl->oikl", wq, w)
                     b = float(scale) * (wq @ b + bq)
                 self.out_ch = w.shape[0]
                 assert self.out_ch <= 16
-                conv3("conv_out", w, b)
-        self.weight_bytes = sum(t.numel() * t.element_size() for t in W.values())
-
-    def _res2d(self, p, x, cin, cout, n, H, Wd, tag, x_stats=None):
-        """ResnetBlock.forward with temb=None (model.py:127-151). Returns (x_out fp32, per-frame GroupNorm stats or None)."""
-        W, pool, AD = self.w, self.pool, self.AD
-        HW, rows = H * Wd, n * H * Wd
-        a = pool.get(f"a{cin}_{rows}", (rows, cin), AD)
-        self._gn(x, n, HW, cin, p + ".n1", 1e-6, True, a, stats=x_stats)
-        h1 = pool.get(f"h{cout}_{rows}", (rows, cout), AD)
-        st, req = self._stats_req(n, cout, HW)
-        ok = ops.conv2d_3x3(a.view(n, H, Wd, cin), W[p + ".c1.w"], ops.make_ep(h1, bias=W[p + ".c1.b"], gn_stats=req))
-        a2 = pool.get(f"a{cout}_{rows}", (rows, cout), AD)
-        self._gn(h1, n, HW, cout, p + ".n2", 1e-6, True, a2, stats=st if ok else None)
-        xs = pool.get(f"{tag}_{cout}_{rows}", (rows, cout), torch.float32)
-        if cin != cout:
-            xa = pool.get(f"xa{cin}_{rows}", (rows, cin), AD)
-            ops.cast_to_act(x, xa)
-            ops.linear(xa, W[p + ".skip.w"], ops.make_ep(xs, bias=W[p + ".skip.b"]))
-            res = xs
-        else:
-            res = x
-        st, req = self._stats_req(n, cout, HW)
-        ok = ops.conv2d_3x3(a2.view(n, H, Wd, cout), W[p + ".c2.w"], ops.make_ep(xs, bias=W[p + ".c2.b"], res1=res, gn_stats=req))
-        return xs, (st if ok else None)
+                self._conv3(sd, "conv_out", (w, b))
 
     def forward_cl(self, x_cl, n, H, Wd, out_nchw):
         """x_cl: act channels-last [n, H, W, 64] (image channels zero-padded); writes float32 NCHW [n, out_ch, H/8, W/8]."""
         W, pool, AD = self.w, self.pool, self.AD
-        self._arena_reset(n)
+        self.arena.reset(n)
         h, hH, hW, hst = None, H, Wd, None
         for i, (kind, p, cin, cout) in enumerate(self.plan):
             rows = n * hH * hW
@@ -288,7 +226,7 @@ class EncoderEngine(DecoderEngine):
                 ok = ops.conv2d_3x3(x_cl, W[p + ".w"], ops.make_ep(h, bias=W[p + ".b"], gn_stats=req))
                 hst = st if ok else None
             elif kind == "res":
-                h, hst = self._res2d(p, h, cin, cout, n, hH, hW, f"s{1 + i % 2}", x_stats=hst)
+                h, hst = self._res2d(p, h, cin, cout, n, hH, hW, f"s{1 + i % 2}", (n, hH * hW), x_stats=hst)
             elif kind == "attn":
                 h = self._attn(p, h, cin, n, hH * hW, x_stats=hst)
                 hst = None
@@ -319,32 +257,21 @@ class Encoder(nn.Module):
                  resamp_with_conv=True, in_channels, resolution=256, z_channels, double_z=True, use_linear_attn=False,
                  attn_type="vanilla", **ignore_kwargs):
         super().__init__()
-
-        def need(cond, what):
-            if not cond:
-                raise NotImplementedError(f"gcd_b200.Encoder: unsupported option ({what}); only the GCD config is built")
-
+        need = need_option("Encoder")
         need(len(attn_resolutions) == 0 and attn_type in ("vanilla", "vanilla-xformers") and not use_linear_attn, "attention")
         need(resamp_with_conv and dropout == 0.0, "resamp_with_conv / dropout")
         need(ch % 64 == 0 and in_channels <= 64 and (2 if double_z else 1) * z_channels <= 16, "channel counts")
         self.cfg = dict(ch=ch, ch_mult=list(ch_mult), num_res_blocks=num_res_blocks, z_channels=z_channels,
                         in_channels=in_channels, double_z=double_z)
         register_param_tree(self, spec.encoder_param_shapes(self.cfg))
-        self._engines = {}
+        self._engines = EngineCache(slots=2)
 
     def invalidate(self):
-        self._engines = {}
+        self._engines.clear()
 
     def engine(self, device, post=None, post_key=None):
         """One packed engine per `post` fold (plain forward / encode_mode), at most two kept; a weight change drops them all."""
-        wk = weights_key(self, device)
-        if getattr(self, "_wkey", None) != wk:
-            self._engines, self._wkey = {}, wk
-        if post_key not in self._engines:
-            if len(self._engines) >= 2:
-                self._engines.pop(next(iter(self._engines)))
-            self._engines[post_key] = EncoderEngine(self.cfg, self.state_dict(), device, post=post)
-        return self._engines[post_key]
+        return self._engines.get(self, device, lambda: EncoderEngine(self.cfg, self.state_dict(), device, post=post), post_key)
 
     def _run(self, x, eng):
         if not x.is_cuda:
@@ -375,18 +302,7 @@ class Encoder(nn.Module):
         return self._run(x, self.engine(x.device, post=post, post_key=pk))
 
 
-def _reference_base():
-    try:
-        from sgm.modules.autoencoding.temporal_ae import VideoDecoder as Ref   # noqa: WPS433
-        return Ref
-    except Exception:
-        return nn.Module
-
-
-_Base = _reference_base()
-
-
-class VideoDecoder(_Base):
+class VideoDecoder(reference_base("sgm.modules.autoencoding.temporal_ae", "VideoDecoder")):
     """Drop-in `target:` for sgm.modules.autoencoding.temporal_ae.VideoDecoder (ctor kwargs: infer_kubric.yaml:152-164)."""
 
     def __init__(self, *args, ch, out_ch, ch_mult=(1, 2, 4, 8), num_res_blocks, attn_resolutions=(), dropout=0.0,
@@ -394,11 +310,7 @@ class VideoDecoder(_Base):
                  use_linear_attn=False, attn_type="vanilla", video_kernel_size=3, alpha=0.0, merge_strategy="learned",
                  time_mode="conv-only", **ignorekwargs):
         nn.Module.__init__(self)   # bypass the reference constructor (it would build the eager torch layers)
-
-        def need(cond, what):
-            if not cond:
-                raise NotImplementedError(f"gcd_b200.VideoDecoder: unsupported option ({what}); only the GCD config is built")
-
+        need = need_option("VideoDecoder")
         need(time_mode == "conv-only" and merge_strategy == "learned", "time_mode/merge_strategy")
         need(len(attn_resolutions) == 0 and attn_type in ("vanilla", "vanilla-xformers") and not use_linear_attn, "attention")
         need(resamp_with_conv and not give_pre_end and not tanh_out and dropout == 0.0, "decoder flags")
@@ -407,21 +319,16 @@ class VideoDecoder(_Base):
         self.cfg = dict(ch=ch, out_ch=out_ch, ch_mult=list(ch_mult), num_res_blocks=num_res_blocks, z_channels=z_channels)
         self.time_mode, self.video_kernel_size, self.alpha, self.merge_strategy = time_mode, video_kernel_size, alpha, merge_strategy
         register_param_tree(self, spec.decoder_param_shapes(self.cfg))
-        self._engine, self._engine_key = None, None
+        self._engines = EngineCache()
 
     def get_last_layer(self, skip_time_mix=False, **kwargs):
         return self.conv_out.time_mix_conv.weight if not skip_time_mix else self.conv_out.weight
 
     def invalidate(self):
-        self._engine, self._engine_key = None, None
+        self._engines.clear()
 
     def engine(self, device):
-        key = weights_key(self, device)
-        if self._engine is None or self._engine_key != key:
-            self._engine = None
-            self._engine = DecoderEngine(self.cfg, self.state_dict(), device)
-            self._engine_key = key
-        return self._engine
+        return self._engines.get(self, device, lambda: DecoderEngine(self.cfg, self.state_dict(), device))
 
     @torch.no_grad()
     def forward(self, z, timesteps=None, skip_video=False, **kwargs):
