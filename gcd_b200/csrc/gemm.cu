@@ -80,7 +80,7 @@ int gcd_make_tmap(CUtensorMap* out, const void* base, int rank, const uint64_t* 
 // ------------------------------------------------------------------------------------------------ kernel
 struct TcParams {
     int ntx, nty, ntz;          // M-tiles along x, y, z
-    int lTW, lTH;               // log2 tile extents (TW*TH*TN == 128)
+    int lTW, lTH;               // log2 tile extents (TW*TH*TN == 128, or 64 under the ping-pong schedule)
     int Xo, Yo, Zo;             // output extents
     int in_mul;
     int ntaps, kchunks;
@@ -103,44 +103,59 @@ struct TcParams {
     long long gn_rpi;
 };
 
-constexpr int TC_A_BYTES = 128 * 128;          // one 128-row x 64-channel activation box, 128B-swizzled
 constexpr int TC_SMEM_MAX = 232448;            // 227 KB opt-in maximum per CTA
 constexpr int TC_THREADS = 384;                // producer warpgroup + two consumer warpgroups
+constexpr int TC_BAR_BYTES = 256;              // full[8], empty[8], turn[2] mbarriers
 
-// residuals: plain loads (the output may alias a residual: each element is read, then written, by the same thread)
-__device__ __forceinline__ float ld_res(const void* base, bool f32, int64_t off) {
-    return f32 ? reinterpret_cast<const float*>(base)[off] : act2f(reinterpret_cast<const act_t*>(base)[off]);
-}
-__device__ __forceinline__ float2 ld_res2(const void* base, bool f32, int64_t off) {
-    if (f32) return *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(base) + off);
-    return unpack2(*reinterpret_cast<const uint32_t*>(reinterpret_cast<const act_t*>(base) + off));
+// residuals: plain loads (the output may alias a residual: each element is read, then written, by the same thread).
+// `p` points at the first of a column pair; the second is read only when it exists (c1ok).
+__device__ __forceinline__ float2 ld_res_pair(const char* p, bool f32, bool c1ok) {
+    if (f32) {
+        if (c1ok) return *reinterpret_cast<const float2*>(p);
+        return make_float2(*reinterpret_cast<const float*>(p), 0.f);
+    }
+    if (c1ok) return unpack2(*reinterpret_cast<const uint32_t*>(p));
+    return make_float2(act2f(*reinterpret_cast<const act_t*>(p)), 0.f);
 }
 
-// One persistent, warp-specialised CTA per SM; the 128-row M-tile is a TW x TH x TN box of output positions.
+// One persistent, warp-specialised CTA per SM; an M-tile is a TW x TH x TN box of output positions.
 //   warpgroup 0 : TMA producer (one thread) — per (tap, 64-channel chunk): one 4-D box of the channels-last activation
 //                 tensor (out-of-range coordinates zero-filled by TMA = conv zero padding) + one 3-D box of BN weight rows,
-//                 both landing 128B-swizzled in shared memory, signalled on an mbarrier ring. It runs ahead into the next
-//                 tile while the consumers are in their epilogue.
-//   warpgroups 1, 2 : consumers — rows [64*(wg-1), +64) of the tile: wgmma m64nBNk16 (fp32 accumulators in registers, one
-//                 batch in flight while the previous stage is released), then the fused epilogue straight from the
-//                 accumulator registers: bias (+ per-row vector) / SiLU / scale / GEGLU / two residual blends, 16-bit or fp32
-//                 stores, and the GroupNorm statistics of the stored values.
+//                 both landing 128B-swizzled in shared memory, signalled on an mbarrier ring. It fills the ring in the
+//                 CTA's tile order and runs ahead as far as the ring allows.
+//   warpgroups 1, 2 : consumers — wgmma m64nBNk16 (fp32 accumulators in registers, one batch in flight while the previous
+//                 stage is released), then the fused epilogue straight from the accumulator registers: bias (+ per-row
+//                 vector) / SiLU / scale / GEGLU / two residual blends, 16-bit or fp32 stores, and the GroupNorm statistics
+//                 of the stored values. Two schedules:
+//     PP = false (cooperative): both work on one 128-row tile, rows [64*cw, +64) each, and run its epilogue together.
+//                 Fewest operand bytes per FLOP from L2; the tensor cores idle during the epilogue.
+//     PP = true (ping-pong): each owns whole 64 x BN tiles (the CTA's tiles with even / odd local index) and they take
+//                 turns on the tensor cores: a warpgroup starts the MMAs of its next tile when the other has issued the
+//                 last MMA of its current one, so one runs its epilogue while the other keeps the tensor pipe busy. A
+//                 warpgroup finds its stages from the global k-step number (local tile index x k-steps per tile + k-step),
+//                 stepping over the stages of the other's tiles. The turn order is also what makes the parity waits on
+//                 `full` unambiguous: when a warpgroup starts a tile, every earlier k-step of the CTA has been filled and
+//                 waited for, so a stage's barrier cannot still be one ring revolution behind the phase it waits on.
+//                 1.67x the operand bytes per FLOP; pays where the epilogue waits on memory (gcd_tc_run chooses).
 // GELU: the `act == 2` (exact erf GELU) instantiation. Kept out of the act 0 / 1 kernels: the erff expansion inside their
 // unrolled epilogue made the UNet's tc_gemm 14 % slower (same registers; one H100 80GB HBM3 at 400 W). The act 0 / 1
 // instantiations compile to the same SASS as without GELU.
-template <int BN, bool GELU>
+template <int BN, bool GELU, bool PP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const TcParams p) {
+    constexpr int TILE_M = PP ? 64 : 128;
+    constexpr int TC_A_BYTES = TILE_M * 128;       // one TILE_M-row x 64-channel activation box, 128B-swizzled
     constexpr int B_BYTES = BN * 128;
     constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES;
     constexpr int NACC = BN / 2;
     extern __shared__ __align__(1024) uint8_t smem[];     // SWIZZLE_128B tiles need 1024-byte alignment
     if ((smem_u32(smem) & 1023u) != 0) __trap();
     const int STAGES = p.stages;
-    float* sStat = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);     // [8 consumer warps][BN][sum, sum of squares]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sStat + (p.gn_stats ? 8 * BN * 2 : 0));
+    float* sStatAll = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // [8 consumer warps][BN][sum, sum of squares]; PP: one [4][BN][2] half per warpgroup
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sStatAll + (p.gn_stats ? 8 * BN * 2 : 0));
     uint64_t* full = bars;                 // [STAGES]
     uint64_t* empty = bars + 8;            // [STAGES]  (STAGES <= 8)
+    uint64_t* turn = bars + 16;            // [2] (PP): turn[w] completes a phase each time warpgroup w may start a main loop
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -149,8 +164,10 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         prefetch_tmap(&mapB);
         for (int i = 0; i < STAGES; i++) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 8);       // one arrival per consumer warp
+            mbar_init(&empty[i], PP ? 4 : 8);   // one arrival per warp that consumed the stage
         }
+        mbar_init(&turn[0], 4);
+        mbar_init(&turn[1], 4);
         fence_barrier_init();
     }
     __syncthreads();
@@ -159,7 +176,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     const int total = m_tiles * p.n_tiles;
     const int kiters = p.ntaps * p.kchunks;
     const int TW = 1 << p.lTW, TH = 1 << p.lTH;
-    const int TN = 128 >> (p.lTW + p.lTH);
+    const int TN = TILE_M >> (p.lTW + p.lTH);
 
     if (warp < 4) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
@@ -190,20 +207,23 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     }
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     // ===================== consumers =====================
-    const int cw = (warp >> 2) - 1;                 // consumer warpgroup: tile rows [64*cw, 64*cw + 64)
-    const int cwarp = warp - 4;                     // consumer warp 0..7
-    const int ct = threadIdx.x - 128;               // consumer thread 0..255
-    const int rl = cw * 64 + (warp & 3) * 16 + (lane >> 2);    // tile row of acc[4i], acc[4i+1]; rl + 8: acc[4i+2], acc[4i+3]
+    const int cw = (warp >> 2) - 1;                 // consumer warpgroup; PP: the CTA's tiles with local index = cw (mod 2)
+    const int a_off = PP ? 0 : cw * (64 * 128);     // cooperative: rows [64*cw, +64) of the 128-row activation box
+    const int rl = (PP ? 0 : cw * 64) + (warp & 3) * 16 + (lane >> 2);   // tile row of acc[4i], acc[4i+1]; rl + 8: acc[4i+2], acc[4i+3]
     const int cb = 2 * (lane & 3);
-    int stage = 0;
-    uint32_t phase = 0;
-    // GroupNorm statistics: consumer thread g < gn_groups owns group g of the current image and flushes it (fp64 atomics)
-    // when the CTA's tile stream moves to another image — tiles of one image are many, the atomics per image few.
+    // statistics party: the threads that share one table and one stream of tiles (a warpgroup under PP, else both)
+    constexpr int ST_WARPS = PP ? 4 : 8, ST_THREADS = ST_WARPS * 32;
+    const int st_t = PP ? (threadIdx.x & 127) : threadIdx.x - 128;
+    const int st_w = PP ? (warp & 3) : warp - 4;
+    const int st_bar = PP ? 1 + cw : 1;
+    float* sStat = sStatAll + (PP ? cw * (4 * BN * 2) : 0);
+    // GroupNorm statistics: party thread g < gn_groups owns group g of the party's current image and flushes it
+    // (fp64 atomics) when its tile stream moves to another image — tiles of one image are many, the atomics per image few.
     int cur_img = -1;
     double st1 = 0.0, st2 = 0.0;
     auto flush = [&]() {
-        if (cur_img >= 0 && ct < p.gn_groups && (st1 != 0.0 || st2 != 0.0)) {
-            double* dst = p.gn_stats + ((int64_t)cur_img * p.gn_groups + ct) * 2;
+        if (cur_img >= 0 && st_t < p.gn_groups && (st1 != 0.0 || st2 != 0.0)) {
+            double* dst = p.gn_stats + ((int64_t)cur_img * p.gn_groups + st_t) * 2;
             atomicAdd(dst, st1);
             atomicAdd(dst + 1, st2);
         }
@@ -211,20 +231,30 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     };
 
     float acc[NACC];
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+    uint32_t turn_parity = cw ^ 1;                  // warpgroup 0 starts at once (parity of the phase before the first)
+    for (int j = PP ? cw : 0;; j += PP ? 2 : 1) {
+        const int tile = blockIdx.x + j * gridDim.x;
+        if (tile >= total) break;
         const int nt = tile % p.n_tiles;
         const int mt = tile / p.n_tiles;
         const int tx = mt % p.ntx;
         const int ty = (mt / p.ntx) % p.nty;
         const int tz = mt / (p.ntx * p.nty);
         const int n0 = nt * BN;
+        const int g0 = j * kiters;                  // global k-step number of the tile's first stage
+        int stage = g0 % STAGES;
+        uint32_t phase = (g0 / STAGES) & 1;
 #pragma unroll
         for (int i = 0; i < NACC; i++) acc[i] = 0.f;
+        if constexpr (PP) {
+            mbar_wait(&turn[cw], turn_parity);
+            turn_parity ^= 1;
+        }
         int prev = -1;
         for (int q = 0; q < kiters; q++) {
             mbar_wait(&full[stage], phase);
             const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-            const uint64_t ad = make_desc_sw128(sa + cw * (64 * 128), 16, 1024);
+            const uint64_t ad = make_desc_sw128(sa + a_off, 16, 1024);
             const uint64_t bd = make_desc_sw128(sa + TC_A_BYTES, 16, 1024);
             wgmma_fence();
 #pragma unroll
@@ -234,6 +264,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 else wgmma_m64n128_ss(acc, ad + 2 * k, bd + 2 * k, 1u);
             }
             wgmma_commit();
+            if (PP && q + 1 == kiters && lane == 0) mbar_arrive(&turn[cw ^ 1]);    // last MMA issued: the other warpgroup's turn
             wgmma_wait<1>();                        // the previous stage's batch is done: release its buffers
             if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
             prev = stage;
@@ -273,49 +304,66 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             }
             continue;
         }
+        const float* bias = p.bias ? p.bias + n0 + cb : nullptr;    // this thread's first column
+        // row base pointers (bytes) of this thread's first column, once per tile; column group i adds 8 * i elements
+        const int eso = p.of32 ? 4 : 2, es1 = p.r1f32 ? 4 : 2, es2 = p.r2f32 ? 4 : 2;
+        char* orow[2];
+        const char* r1row[2];
+        const char* r2row[2];
         const float* rv[2] = {nullptr, nullptr};
-        if (p.rowvec) {
 #pragma unroll
-            for (int h = 0; h < 2; h++)
-                if (grow[h] >= 0) rv[h] = p.rowvec + (grow[h] / p.rpv) * (int64_t)p.ldv;
+        for (int h = 0; h < 2; h++) {
+            const int64_t g = grow[h] < 0 ? 0 : grow[h];
+            orow[h] = reinterpret_cast<char*>(p.out) + (g * p.ldo + n0 + cb) * eso;
+            r1row[h] = reinterpret_cast<const char*>(p.res1) + (g * p.ld1 + n0 + cb) * es1;
+            r2row[h] = reinterpret_cast<const char*>(p.res2) + (g * p.ld2 + n0 + cb) * es2;
+            if (p.rowvec && grow[h] >= 0) rv[h] = p.rowvec + (grow[h] / p.rpv) * (int64_t)p.ldv + n0 + cb;
         }
         const bool stats = p.gn_stats != nullptr;
+        const bool has1 = p.res1 != nullptr, has2 = p.res2 != nullptr;
+        // residuals of column group i are loaded one group ahead of the arithmetic that uses them
+        float2 t1[2], t2[2];
+        auto load_res = [&](int i, float2 (&a)[2], float2 (&b)[2]) {
+            const int col = n0 + 8 * i + cb;
+            if (col >= p.N) return;
+            const bool c1ok = col + 1 < p.N;
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                if (grow[h] < 0) continue;
+                if (has1) a[h] = ld_res_pair(r1row[h] + 8 * i * es1, p.r1f32, c1ok);
+                if (has2) b[h] = ld_res_pair(r2row[h] + 8 * i * es2, p.r2f32, c1ok);
+            }
+        };
+        t1[0] = t1[1] = t2[0] = t2[1] = make_float2(0.f, 0.f);
+        load_res(0, t1, t2);
 #pragma unroll
         for (int i = 0; i < BN / 8; i++) {
             const int col = n0 + 8 * i + cb;
             const bool c0ok = col < p.N, c1ok = col + 1 < p.N;
+            float2 u1[2] = {t1[0], t1[1]}, u2[2] = {t2[0], t2[1]};
+            if (i + 1 < BN / 8) load_res(i + 1, t1, t2);
             float s1a = 0.f, s2a = 0.f, s1b = 0.f, s2b = 0.f;   // statistics of columns col, col + 1 over this thread's rows
             if (c0ok) {
                 float2 b = make_float2(0.f, 0.f);
-                if (p.bias) b = c1ok ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(__ldg(p.bias + col), 0.f);
+                if (bias) b = c1ok ? __ldg(reinterpret_cast<const float2*>(bias + 8 * i)) : make_float2(__ldg(bias + 8 * i), 0.f);
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
                     if (grow[h] < 0) continue;
                     float v0 = acc[4 * i + 2 * h] + b.x, v1 = acc[4 * i + 2 * h + 1] + b.y;
-                    if (rv[h]) { v0 += rv[h][col]; if (c1ok) v1 += rv[h][col + 1]; }
+                    if (rv[h]) { v0 += rv[h][8 * i]; if (c1ok) v1 += rv[h][8 * i + 1]; }
                     if constexpr (GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
                     else if (p.act == 1) { v0 = silu(v0); v1 = silu(v1); }
                     v0 *= p.a0; v1 *= p.a0;
-                    if (p.res1) {
-                        const int64_t o = grow[h] * p.ld1 + col;
-                        if (c1ok) { const float2 t = ld_res2(p.res1, p.r1f32, o); v0 += p.a1 * t.x; v1 += p.a1 * t.y; }
-                        else v0 += p.a1 * ld_res(p.res1, p.r1f32, o);
-                    }
-                    if (p.res2) {
-                        const int64_t o = grow[h] * p.ld2 + col;
-                        if (c1ok) { const float2 t = ld_res2(p.res2, p.r2f32, o); v0 += p.a2 * t.x; v1 += p.a2 * t.y; }
-                        else v0 += p.a2 * ld_res(p.res2, p.r2f32, o);
-                    }
-                    const int64_t o = grow[h] * p.ldo + col;
+                    if (has1) { v0 += p.a1 * u1[h].x; if (c1ok) v1 += p.a1 * u1[h].y; }
+                    if (has2) { v0 += p.a2 * u2[h].x; if (c1ok) v1 += p.a2 * u2[h].y; }
+                    char* o = orow[h] + 8 * i * eso;
                     if (p.of32) {
-                        float* out = reinterpret_cast<float*>(p.out);
-                        if (c1ok) *reinterpret_cast<float2*>(out + o) = make_float2(v0, v1);
-                        else out[o] = v0;
+                        if (c1ok) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+                        else *reinterpret_cast<float*>(o) = v0;
                     } else {
-                        act_t* out = reinterpret_cast<act_t*>(p.out);
                         const uint32_t w = pack2(v0, v1);
-                        if (c1ok) *reinterpret_cast<uint32_t*>(out + o) = w;
-                        else out[o] = f2act(v0);
+                        if (c1ok) *reinterpret_cast<uint32_t*>(o) = w;
+                        else *reinterpret_cast<act_t*>(o) = f2act(v0);
                         const float2 r = unpack2(w);             // statistics of the stored (rounded) values
                         v0 = r.x; v1 = r.y;
                     }
@@ -330,29 +378,30 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     s1b += __shfl_xor_sync(0xffffffffu, s1b, off); s2b += __shfl_xor_sync(0xffffffffu, s2b, off);
                 }
                 if (lane < 4) {
-                    float* d = sStat + (cwarp * BN + 8 * i + cb) * 2;
+                    float* d = sStat + (st_w * BN + 8 * i + cb) * 2;
                     d[0] = s1a; d[1] = s2a; d[2] = s1b; d[3] = s2b;
                 }
             }
         }
         if (stats) {
-            // fixed summation order (warps, then columns of the group): the statistics do not depend on scheduling
-            named_bar_sync(1, 256);
-            if (ct < BN) {
+            // fixed summation order (warps, then columns of the group): the statistics do not depend on scheduling.
+            // The barrier spans the statistics party only: under PP the other warpgroup is in its main loop.
+            named_bar_sync(st_bar, ST_THREADS);
+            for (int c = st_t; c < BN; c += ST_THREADS) {
                 float a = 0.f, b = 0.f;
 #pragma unroll
-                for (int w = 0; w < 8; w++) { a += sStat[(w * BN + ct) * 2]; b += sStat[(w * BN + ct) * 2 + 1]; }
-                sStat[ct * 2] = a; sStat[ct * 2 + 1] = b;
+                for (int w = 0; w < ST_WARPS; w++) { a += sStat[(w * BN + c) * 2]; b += sStat[(w * BN + c) * 2 + 1]; }
+                sStat[c * 2] = a; sStat[c * 2 + 1] = b;
             }
-            named_bar_sync(1, 256);
+            named_bar_sync(st_bar, ST_THREADS);
             const int64_t row0 = ((int64_t)(tz * TN) * p.Yo + ty * TH) * p.Xo + tx * TW;
             const int img = (int)(row0 / p.gn_rpi);
             if (img != cur_img) { flush(); cur_img = img; }
-            if (ct < p.gn_groups) {
-                const int lo = max(ct * p.gn_cpg, n0), hi = min(min((ct + 1) * p.gn_cpg, n0 + BN), p.N);
+            if (st_t < p.gn_groups) {
+                const int lo = max(st_t * p.gn_cpg, n0), hi = min(min((st_t + 1) * p.gn_cpg, n0 + BN), p.N);
                 for (int c = lo; c < hi; c++) { st1 += (double)sStat[(c - n0) * 2]; st2 += (double)sStat[(c - n0) * 2 + 1]; }
             }
-            named_bar_sync(1, 256);                 // sStat is rewritten by the next tile
+            named_bar_sync(st_bar, ST_THREADS);     // sStat is rewritten by the next tile
         }
     }
     if (p.gn_stats) flush();
@@ -370,15 +419,15 @@ static int num_sms_cached() {
     return n;
 }
 
-template <int BN, bool GELU>
+template <int BN, bool GELU, bool PP>
 static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, TcParams& p, cudaStream_t st) {
     static bool configured = false;
     if (!configured) {
-        GCD_CUDA_CHECK(cudaFuncSetAttribute(tc_gemm_kernel<BN, GELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
+        GCD_CUDA_CHECK(cudaFuncSetAttribute(tc_gemm_kernel<BN, GELU, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
         configured = true;
     }
-    constexpr int STAGE_BYTES = TC_A_BYTES + BN * 128;
-    const int fixed = (p.gn_stats ? 8 * BN * 2 * 4 : 0) + 256;     // statistics table + barriers
+    constexpr int STAGE_BYTES = (PP ? 64 : 128) * 128 + BN * 128;
+    const int fixed = (p.gn_stats ? 8 * BN * 2 * 4 : 0) + TC_BAR_BYTES;     // statistics tables + barriers
     int stages = (TC_SMEM_MAX - fixed) / STAGE_BYTES;
     if (stages > 8) stages = 8;
     GCD_REQUIRE(stages >= 2, "tc_gemm: not enough shared memory for the pipeline (BN=%d)", BN);
@@ -388,7 +437,7 @@ static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, TcParams& p, 
     const int sms = num_sms_cached();
     GCD_REQUIRE(sms > 0, "tc_gemm: no CUDA device");
     const int grid = tiles < sms ? tiles : sms;
-    tc_gemm_kernel<BN, GELU><<<grid, TC_THREADS, smem, st>>>(mA, mB, p);
+    tc_gemm_kernel<BN, GELU, PP><<<grid, TC_THREADS, smem, st>>>(mA, mB, p);
     GCD_CUDA_CHECK(cudaGetLastError());
     g_launches++;
     return 0;
@@ -453,22 +502,28 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
 
     TcParams p;
     memset(&p, 0, sizeof(p));
+    // ---- schedule. Ping-pong hides an epilogue that waits on memory (residual reads, fp32 stores) behind the other
+    // warpgroup's MMAs, at 1.67x the operand bytes per FLOP from L2. Measured per op of the UNet forward and the VAE decode on
+    // one H100 80GB HBM3 at a 700 W limit: ops with a residual or an fp32 output 14-40 % faster under ping-pong, plain 16-bit
+    // stores within a few per cent either way; the GEGLU GEMMs already run at 420-600 TFLOP/s cooperatively (DESIGN.md §6).
+    const bool pp = !e.geglu && (e.res1 || e.res2 || e.out_f32);
+    const int TILE_M = pp ? 64 : 128;
     // ---- tile search
     int TW, TH, TN;
     if (op->gemm_tile) {
-        TW = 128; TH = 1; TN = 1;
+        TW = TILE_M; TH = 1; TN = 1;
     } else {
         TW = 1;
-        while (TW < 128 && op->Xo % (TW * 2) == 0) TW *= 2;
+        while (TW < TILE_M && op->Xo % (TW * 2) == 0) TW *= 2;
         long best = -1;
         int bestTH = 1;
-        for (int th = 1; th * TW <= 128; th *= 2) {
-            int tn = 128 / (TW * th);
+        for (int th = 1; th * TW <= TILE_M; th *= 2) {
+            int tn = TILE_M / (TW * th);
             long cov = (long)((op->Yo + th - 1) / th) * th * (long)((op->Zo + tn - 1) / tn) * tn;
             if (best < 0 || cov <= best) { best = cov; bestTH = th; }
         }
         TH = bestTH;
-        TN = 128 / (TW * TH);
+        TN = TILE_M / (TW * TH);
     }
     p.lTW = ilog2(TW);
     p.lTH = ilog2(TH);
@@ -485,8 +540,8 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
     GCD_REQUIRE(!p.w_batched || TH == 1, "gcd_tc_run: batched weights need gemm tiling");
 
     // Tile width: the widest wgmma (N = 256) reads each activation tile once per 256 output columns; N = 320 / 640 / 1280
-    // convs split evenly into 160-column tiles. On small problems (the 9x16 / 18x32 levels: M = 4032 rows) wave quantisation
-    // over the SMs decides instead: cost = waves x tile width.
+    // convs split evenly into 160-column tiles. On small problems (the 9x16 / 18x32 levels: M = 4032 rows = 63 M-tiles) wave
+    // quantisation over the SMs decides instead: cost = waves x tile width.
     int BN;
     if (op->N % 256 == 0 || op->N >= 384) BN = 256;
     else if (op->N % 160 == 0) BN = 160;
@@ -510,7 +565,8 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
     if (e.res2 && check_ep_tensor(e.res2, e.res2_f32, e.ld_res2, "res2")) return -2;
     int stats_skipped = 0;
     if (e.gn_stats) {
-        GCD_REQUIRE(e.gn_cpg > 0 && e.gn_groups > 0 && e.gn_rows_per_img > 0 && !e.geglu, "gcd_tc_run: bad gn_stats arguments");
+        GCD_REQUIRE(e.gn_cpg > 0 && e.gn_groups > 0 && e.gn_groups <= 128 && e.gn_rows_per_img > 0 && !e.geglu,
+                    "gcd_tc_run: bad gn_stats arguments (at most 128 groups: one thread of a consumer warpgroup per group)");
         const long long rpi = e.gn_rows_per_img, plane = (long long)op->Xo * op->Yo;
         const bool full = (op->Xo % TW == 0) && (op->Yo % TH == 0) && (op->Zo % TN == 0);
         const bool one_img = TN == 1 && ((rpi % plane == 0) || (TH == 1 && rpi % TW == 0 && (op->Xo % rpi == 0 || rpi % op->Xo == 0)));
@@ -559,10 +615,14 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
     tmap_cache_put(tkey, ts);
     }
     int rc;
+#define GCD_TC_LAUNCH(bn)                                                                                  \
+    (e.act == 2 ? (pp ? launch_tc<bn, true, true>(mA, mB, p, st) : launch_tc<bn, true, false>(mA, mB, p, st)) \
+                : (pp ? launch_tc<bn, false, true>(mA, mB, p, st) : launch_tc<bn, false, false>(mA, mB, p, st)))
     switch (BN) {
-        case 256: rc = e.act == 2 ? launch_tc<256, true>(mA, mB, p, st) : launch_tc<256, false>(mA, mB, p, st); break;
-        case 160: rc = e.act == 2 ? launch_tc<160, true>(mA, mB, p, st) : launch_tc<160, false>(mA, mB, p, st); break;
-        default: rc = e.act == 2 ? launch_tc<128, true>(mA, mB, p, st) : launch_tc<128, false>(mA, mB, p, st); break;
+        case 256: rc = GCD_TC_LAUNCH(256); break;
+        case 160: rc = GCD_TC_LAUNCH(160); break;
+        default: rc = GCD_TC_LAUNCH(128); break;
     }
+#undef GCD_TC_LAUNCH
     return rc ? rc : stats_skipped;
 }

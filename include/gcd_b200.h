@@ -54,7 +54,7 @@ typedef struct gcd_epilogue {
     int32_t act;
     /* Optional fused GroupNorm statistics of the tensor being written (the NEXT GroupNorm's input):
      * gn_stats[(row / gn_rows_per_img) * gn_groups + col / gn_cpg][0..1] += (sum, sum of squares) of the stored values.
-     * Zero the buffer first. Only produced when every 128-row output tile lies inside one statistics image and all
+     * Zero the buffer first. Only produced when every output tile (64 rows for ops with a residual or an fp32 output, else 128) lies inside one statistics image and all
      * tiles are full; otherwise gcd_tc_run returns 1 (success, statistics NOT produced: run gcd_groupnorm_stats). */
     double* gn_stats;
     int32_t gn_cpg;
@@ -75,7 +75,7 @@ typedef struct gcd_tc_op {
     int32_t in_mul;            /* 1, or 2 for stride-2 conv */
     int32_t ntaps;             /* 1..9 */
     int8_t tap_dx[9], tap_dy[9], tap_dz[9];
-    int32_t gemm_tile;         /* 1: plain GEMM tiling (128 consecutive x), 0: search conv tile */
+    int32_t gemm_tile;         /* 1: plain GEMM tiling (one tile = consecutive x), 0: search conv tile */
     const void* W;             /* [N, ldw] act, K-contiguous, ldw >= ntaps*C ; batched over y if w_batch_stride != 0 */
     int64_t ldw;
     int64_t w_batch_stride;    /* elements between per-y weight matrices (batched GEMM), else 0 */

@@ -1,0 +1,117 @@
+"""GPU parity tests of tc_gemm's ping-pong schedule (ops with a residual or an fp32 output) at the edges of its 64-row tile geometry,
+and of the cooperative 128-row schedule (plain 16-bit output) on the same problems: tile counts that leave one
+consumer warpgroup without work or with one tile more than the other, k-step counts that do not divide the stage ring, and
+fused GroupNorm statistics whose image boundary is a 64-row but not a 128-row boundary. Same references as test_ops_gpu.py:
+plain torch fp32 math on the same (16-bit rounded) inputs."""
+import pytest
+import torch
+import torch.nn.functional as F
+
+pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(scope="module")
+def ops():
+    from gcd_b200 import ops as o
+    o.lib()
+    return o
+
+
+def rnd(*shape, scale=1.0, dtype=None, seed=[1000]):
+    seed[0] += 1
+    g = torch.Generator().manual_seed(seed[0])
+    t = torch.randn(*shape, generator=g) * scale
+    return t.cuda() if dtype is None else t.to(dtype).cuda()
+
+
+def relerr(a, b):
+    a, b = a.float(), b.float()
+    return ((a - b).norm() / (b.norm() + 1e-30)).item()
+
+
+def _sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+# (M, K, N): M in 64-row tiles x N in 256 / 160 / 128-column tiles gives the tile count; with one CTA per SM a CTA runs
+# ceil or floor of tiles / SMs of them, alternating between its two consumer warpgroups.
+@pytest.mark.parametrize("M,K,N", [
+    (64, 320, 256),                 # exactly one tile: the second warpgroup has none
+    (3 * 64, 64, 256),              # odd tile count below the SM count; one k-step per tile
+    (5 * 64 - 7, 5 * 64, 256),      # five k-steps with BN = 256 (five stages): every tile starts on stage 0
+    (64 * 7, 7 * 64, 512),          # seven k-steps over five stages: tiles start on every stage, both ring phases
+    (64 * 3, 3 * 64, 160),          # BN = 160 (eight stages), fewer k-steps than stages
+    (64 * 5, 11 * 64, 128),         # BN = 128 (eight stages), more k-steps than stages
+])
+@pytest.mark.parametrize("out_f32", [True, False])
+def test_linear_tile_edges(ops, M, K, N, out_f32):
+    AD = ops.act_dtype()
+    x, w = rnd(M, K, dtype=AD), rnd(N, K, scale=K ** -0.5, dtype=AD)
+    bias = rnd(N)
+    out = torch.empty(M, N, device="cuda", dtype=torch.float32 if out_f32 else AD)
+    ops.linear(x, w, ops.make_ep(out, bias=bias))
+    ref = x.float() @ w.float().t() + bias
+    assert relerr(out, ref) < (2e-5 if out_f32 else 1e-3)
+
+
+@pytest.mark.parametrize("extra", [1, 2])
+def test_linear_odd_tiles_above_sm_count(ops, extra):
+    """2 x SMs + 1 and 3 x SMs + 2 tiles: some CTAs run three tiles (two on warpgroup 0, one on warpgroup 1), with both
+    residuals and the in-place update that the UNet's residual stream uses."""
+    AD = ops.act_dtype()
+    tiles = (1 + extra) * _sms() + extra
+    M, K, N = tiles * 64 - 13, 192, 256
+    x, w = rnd(M, K, dtype=AD), rnd(N, K, scale=K ** -0.5, dtype=AD)
+    bias, r1, r2 = rnd(N), rnd(M, N), rnd(M, N, dtype=AD)
+    h = r1.clone()
+    ops.linear(x, w, ops.make_ep(h, bias=bias, res1=h, a_res1=0.5, res2=r2, a_res2=0.25))
+    ref = x.float() @ w.float().t() + bias + 0.5 * r1 + 0.25 * r2.float()
+    assert relerr(h, ref) < 2e-5
+
+
+def test_linear_geglu_odd_tiles(ops):
+    AD = ops.act_dtype()
+    M, K, C4 = 64 * 3 + 5, 320, 384
+    x = rnd(M, K, dtype=AD)
+    w = rnd(2 * C4, K, scale=K ** -0.5, dtype=AD)
+    b = rnd(2 * C4)
+    idx = torch.arange(2 * C4).view(2, C4 // 16, 16).permute(1, 0, 2).reshape(-1).cuda()   # 16 value / 16 gate blocks
+    out = torch.empty(M, C4, device="cuda", dtype=AD)
+    ops.linear(x, w[idx].contiguous(), ops.make_ep(out, bias=b[idx].contiguous(), geglu=True))
+    y = x.float() @ w.float().t() + b
+    assert relerr(out, y[:, :C4] * F.gelu(y[:, C4:])) < 1.5e-3
+
+
+@pytest.mark.parametrize("G,M", [(3, 64), (5, 200), (7, 100)])
+def test_bmm_nt_odd_batch(ops, G, M):
+    AD = ops.act_dtype()
+    K, N = 192, 300
+    a, b = rnd(G, M, K, dtype=AD), rnd(G, N, K, scale=K ** -0.5, dtype=AD)
+    out = torch.empty(G * M, N, device="cuda")
+    ops.bmm_nt(a, b, ops.make_ep(out))
+    ref = torch.bmm(a.float(), b.float().transpose(1, 2)).reshape(G * M, N)
+    assert relerr(out, ref) < 2e-5
+
+
+@pytest.mark.parametrize("n,H,W", [(3, 3, 64), (5, 1, 64), (2, 9, 16), (3, 22, 32)])
+@pytest.mark.parametrize("out_f32", [True, False])
+def test_fused_groupnorm_stats_64_row_images(ops, n, H, W, out_f32):
+    """Images of an odd number of 64-row tiles: every second image boundary falls inside what a 128-row tile would cover.
+    Each consumer warpgroup keeps its own per-image sums and flushes them when its own tile stream changes image."""
+    AD = ops.act_dtype()
+    C, Co = 64, 320
+    x = rnd(n, H, W, C, dtype=AD)
+    wp = rnd(Co, 9 * C, scale=(9 * C) ** -0.5, dtype=AD)
+    bias = rnd(Co)
+    out = torch.empty(n * H * W, Co, device="cuda", dtype=torch.float32 if out_f32 else AD)
+    st = torch.zeros(n * 64, device="cuda", dtype=torch.float64)
+    produced = ops.conv2d_3x3(x, wp, ops.make_ep(out, bias=bias, gn_stats=(st, Co // 32, 32, H * W)))
+    w4 = wp.float().view(Co, 3, 3, C).permute(0, 3, 1, 2)
+    ref_out = F.conv2d(x.float().permute(0, 3, 1, 2), w4, bias, padding=1).permute(0, 2, 3, 1).reshape(n * H * W, Co)
+    assert relerr(out, ref_out) < (3e-5 if out_f32 else 1e-3)
+    if out_f32 and (H * W) % 64 == 0:              # fp32 output: 64-row tiles, one image per tile
+        assert produced
+    if produced:
+        v = out.double().view(n, H * W, 32, Co // 32)
+        ref = torch.stack([v.sum((1, 3)), (v * v).sum((1, 3))], -1).reshape(-1)
+        assert torch.allclose(st, ref, rtol=1e-5, atol=1e-3)

@@ -1,7 +1,8 @@
-"""Autotune study of `tc_gemm_kernel`'s tile width / cluster mode per op of the hot path (experiments, on an H100; the cluster-mode argument is ignored by the Hopper kernel).
+"""Autotune study of `tc_gemm_kernel`'s tile width per op of the hot path (experiments, on an H100; the schedule, cooperative or ping-pong, follows
+from the op's epilogue inside gcd_tc_run, so the tile width BN is the only thing to choose).
 
 Records every `gcd_tc_run` descriptor of one full-size CFG forward + one VAE decode, then re-issues each DISTINCT op (same buffers,
-same fused epilogue) under every (BN, mode) the kernel supports — `gcd_tc_override` — and times it with CUDA events (median of 7,
+same fused epilogue) under every BN the kernel supports — `gcd_tc_override` — and times it with CUDA events (median of 7,
 back to back; the level-1 operands exceed the L2). Prints, per op, the automatic choice's time, the best configuration and the gain,
 and the total over the forward weighted by how often the op occurs. Output: gpurun_out/autotune_tc.json.
 """
@@ -114,22 +115,21 @@ if TOP > 0:                           # rank the UNet ops by a quick burst timin
     order = [(k, v) for k, v in order if k in keep]
     SUSTAIN = sus
 for key, (o, cnt) in order:
-    if key[-1]:                       # batched weights: single-CTA mode only
+    if key[-1]:                       # batched weights (bmm_nt): not on the hot path's critical ops
         continue
     L.gcd_tc_override(0, 0)
     t_auto = timeit(o)
     best = (t_auto, "auto")
     res = {}
     for bn in ((256,) if key[6] else (128, 160, 256)):
-        for mode in (2, 3):
-            L.gcd_tc_override(bn, mode)
-            rc = real(ctypes.byref(o), st)
-            if rc < 0:
-                continue
-            t = timeit(o)
-            res[f"bn{bn}m{mode}"] = round(t, 4)
-            if t < best[0]:
-                best = (t, f"bn{bn}m{mode}")
+        L.gcd_tc_override(bn, 0)
+        rc = real(ctypes.byref(o), st)
+        if rc < 0:
+            continue
+        t = timeit(o)
+        res[f"bn{bn}"] = round(t, 4)
+        if t < best[0]:
+            best = (t, f"bn{bn}")
     L.gcd_tc_override(0, 0)
     part = key[0]
     tot_auto[part] += t_auto * cnt

@@ -28,5 +28,25 @@ for name, fn in (("unet_2steps", lambda: pipe.sample_latents(x.clone(), c, uc)),
     for k, d in rows[:45]:
         print(f"{d['ms']:8.2f} ms  x{d['launches']:4d}  {d['flops']/max(d['ms'],1e-9)/1e9:7.0f} TF  {d['bytes']/max(d['ms'],1e-9)/1e6:7.0f} GB/s  {k}")
     out[name] = {"wall_ms": tot, "classes": {k: d for k, d in rows}}
+# Practical ceiling of this card at its power limit: cuBLAS fp16 at three of the UNet's linear shapes (a yardstick for the table
+# above only; nothing in the package calls cuBLAS).
+out["cublas_ceiling"] = {}
+for M, K, N in ((258048, 320, 2560), (258048, 1280, 320), (64512, 640, 5120)):
+    a = torch.randn(M, K, device=dev, dtype=torch.float16)
+    b = torch.randn(N, K, device=dev, dtype=torch.float16)
+    for _ in range(5):
+        torch.matmul(a, b.t())
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(20):
+        torch.matmul(a, b.t())
+    e1.record(); torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1) / 20
+    print(f"cuBLAS fp16 M{M} N{N} K{K}: {ms:.3f} ms  {2.0 * M * N * K / ms / 1e9:.0f} TF")
+    out["cublas_ceiling"][f"M{M} N{N} K{K}"] = {"ms": ms, "tflops": 2.0 * M * N * K / ms / 1e9}
+    del a, b
+import subprocess
+print("card:", torch.cuda.get_device_name(0), "power limit:", subprocess.run(
+    ["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip())
 os.makedirs("gpurun_out", exist_ok=True)
 json.dump(out, open("gpurun_out/prof_forward.json", "w"), indent=1)
