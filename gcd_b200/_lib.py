@@ -71,6 +71,8 @@ _SIGS = {
     "gcd_timestep_embedding": (c_int, [c_void_p, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),
     "gcd_spherical_embed": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "gcd_frame_metrics": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "gcd_render_views": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                 c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "gcd_sampler_prep": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "gcd_sampler_update": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
                                    c_float, c_void_p, c_void_p]),

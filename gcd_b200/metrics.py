@@ -64,7 +64,15 @@ def calculate_metrics(gt_rgb, reproject_rgb, pred_samples_rgb):
     out = {k: torch.stack(v) for k, v in acc.items()}                     # (S, T)
     for k in keys:
         out[k.replace("frame_", "mean_")] = torch.nanmean(out[k], dim=1)  # (S)
-    unc = pred_samples_rgb.float().std(dim=0, unbiased=False).mean(dim=1)  # np.std(axis=0) then nanmean over channels: (T, H, W)
+    std = pred_samples_rgb.float().std(dim=0, unbiased=False)               # np.std(axis=0): (T, 3, H, W)
+    unc = std.mean(dim=1)                                                   # then nanmean over channels: (T, H, W)
     out["frame_diversity"] = unc.mean(dim=(1, 2)).double().cpu()
     out["mean_diversity"] = out["frame_diversity"].mean()
+    if vis is not None:                    # test.py:470-480: the per-sample std over the masked pixels of each frame
+        for name, m in (("vis", vis), ("occ", occ)):
+            num = (std.double() * m[:, None]).sum(dim=(1, 2, 3))
+            den = 3.0 * m.sum(dim=(1, 2)).double()
+            fd = torch.where(den > 0, num / den.clamp(min=1), torch.full_like(num, float("nan"))).cpu()
+            out[f"frame_diversity_{name}"] = fd
+            out[f"mean_diversity_{name}"] = torch.nanmean(fd)
     return out, unc

@@ -398,6 +398,21 @@ def sampler_update(x, net_out, ld_net, BT, T, H, W, c_out, c_skip, sigma, dt, sc
                                        float(dt), _p(scale), _stream()), "sampler_update")
 
 
+def render_views(xyz, rgb, segm, palette, desc, cams, H, W, Hp, Wp, spread_radius, acc, maxd, out):
+    """Point-cloud renders (include/gcd_b200.h gcd_render_views). xyz fp16 [F, P, 3], rgb uint8 [F, P, 3], segm uint8 [F, P] + palette
+    float32 [256, 3] or both None; desc int32 [R, 4] (CPU), cams float64 [R, 24] (device); acc float64 [R, H*W, 4] and maxd float64
+    [R] workspaces; out float32 [R, 3, Hp, Wp]."""
+    _need_cuda(xyz, rgb, segm, palette, cams, acc, maxd, out)
+    assert xyz.dtype == torch.float16 and rgb.dtype == torch.uint8 and xyz.is_contiguous() and rgb.is_contiguous()
+    assert desc.dtype == torch.int32 and not desc.is_cuda and desc.is_contiguous()
+    R, P = desc.shape[0], xyz.shape[1]
+    d_desc = desc.to(xyz.device, non_blocking=False)
+    n = int(desc[:, 2].sum())
+    with _timed("render", 0.0, n * 10 + R * H * W * 32 * 3 + out.numel() * 4):
+        check(lib().gcd_render_views(_p(xyz), _p(rgb), _p(segm), _p(palette), P, R, _p(desc), _p(d_desc), _p(cams), H, W, Hp, Wp,
+                                     int(spread_radius), _p(acc), _p(maxd), _p(out), _stream()), "render_views")
+
+
 _REPLAYED = 0
 
 

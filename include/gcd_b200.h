@@ -195,6 +195,22 @@ void gcd_tc_override(int bn, int mode);
  * sums over the 3 channels. PSNR = 10 log10(count / sum) for data_range 1; SSIM = sum / count. */
 int gcd_frame_metrics(const float* pred, const float* gt, const uint8_t* mask, int frames, int H, int W, double* out, void* stream);
 
+/* Point-cloud view synthesis of the evaluation clips (gcd-model/sgm/data/geometry.py:242-444 project_points_to_pixels +
+ * spreaded_index_add + blur_into_black, then the bilinear resize and `* 2 - 1` of kubric_arbit.py:410-563 / pardom_arbit.py:585-738).
+ * R renders in one call. Render r reads points [desc[r].p0, desc[r].p0 + desc[r].n) of frame desc[r].frame:
+ *   xyz: fp16 [frames, P, 3] world coordinates (non-finite allowed: such points are dropped); rgb: uint8 [frames, P, 3];
+ *   segm: uint8 [frames, P] semantic ids with palette float32 [256, 3], or both NULL. With segm, colour = (1 - a) rgb/255 + a palette[id]
+ *   in fp32 with a = cams[r][21].
+ *   desc: int32 [R, 4] = {frame, p0, n, blur kernel (odd, 1..31; sigma = k / 4)}, on the device; desc_host: the same array on the host.
+ *   cams: fp64 [R, 24] on the device = {K (3x3 row-major, pixel units), RT[0:3, 0:3] (row-major), RT[0:3, 3], a, 0, 0}.
+ * Render size H x W, output size Hp x Wp; spread_radius 0..8 (spreaded_index_add's offsets, weight x 0.02).
+ * acc: fp64 [R, H*W, 4] workspace and maxd: fp64 [R], both zeroed here. On return maxd[r] is the largest depth of the render's valid
+ * points, 0 when no point lands in the image (out is then the all-black render; the caller reports the error).
+ * out: float32 [R, 3, Hp, Wp] in [-1, 1]. Errors: -2 bad arguments (null pointer, point range, kernel size, blur radius >= H or W). */
+int gcd_render_views(const void* xyz, const uint8_t* rgb, const uint8_t* segm, const float* palette, int64_t P, int R,
+                     const int32_t* desc_host, const int32_t* desc, const double* cams, int H, int W, int Hp, int Wp,
+                     int spread_radius, double* acc, double* maxd, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
