@@ -11,6 +11,7 @@ that module tree for the parts this package replaces, so the same call works and
     first_stage_model.quant_conv.*               1x1 conv of AutoencoderKL (folded into Encoder.encode_mode)
     model_ema.*                                  LitEma shadows of `model` (modules/ema.py: name with the dots removed)
     conditioner.embedders.<i>.*                  gcd_b200.embedders (optional, HotPathRoot(conditioner=...))
+    lpips.*                                      gcd_b200.lpips.LPIPS (optional, HotPathRoot(lpips=...))
 
 Host-side plumbing only: no kernels involved; the modules repack their weights for the CUDA engines on the next forward
 (gcd_b200.engine.weights_key).
@@ -47,18 +48,22 @@ class HotPathRoot(nn.Module):
     """Module tree with the DiffusionEngine's attribute names for the replaced components (everything else in a checkpoint —
     conditioner, loss, optimizer — lands in `unexpected`, exactly like unknown keys do in the reference's strict=False load)."""
 
-    def __init__(self, unet, decoder, encoder=None, conditioner=None):
+    def __init__(self, unet, decoder, encoder=None, conditioner=None, lpips=None):
         """`conditioner`: optional embedder modules in YAML order (gcd_b200.embedders.build_embedders), registered as
         `conditioner.embedders.<i>` — GeneralConditioner's attribute names — so the CLIP tower
         (`conditioner.embedders.0.open_clip.model.*`), the conditioning-frame encoder (`...3.encoder.{encoder,quant_conv}.*`)
         and the spherical embedder (`...5.proj.*`) load through the same call. The decoder half of that autoencoder
-        (`...3.encoder.{decoder,post_quant_conv}.*`) has no module here and stays in `unexpected`."""
+        (`...3.encoder.{decoder,post_quant_conv}.*`) has no module here and stays in `unexpected`.
+        `lpips`: optional gcd_b200.lpips.LPIPS, registered as `lpips` (DiffusionEngine.lpips, models/diffusion.py:187), so the
+        `lpips.*` tensors load too."""
         super().__init__()
         self.model = sampling.OpenAIWrapper(unet)
         self.first_stage_model = _FirstStage(decoder, encoder)
         if conditioner is not None:
             self.conditioner = nn.Module()
             self.conditioner.embedders = nn.ModuleList(list(conditioner))
+        if lpips is not None:
+            self.lpips = lpips
 
     def init_from_ckpt(self, path, use_ema=False):
         """models/diffusion.py:191-219. Returns (missing, unexpected); with use_ema the `model_ema.*` shadows overwrite the

@@ -137,10 +137,11 @@ __device__ __forceinline__ float2 ld_res_pair(const char* p, bool f32, bool c1ok
 //                 `full` unambiguous: when a warpgroup starts a tile, every earlier k-step of the CTA has been filled and
 //                 waited for, so a stage's barrier cannot still be one ring revolution behind the phase it waits on.
 //                 1.67x the operand bytes per FLOP; pays where the epilogue waits on memory (gcd_tc_run chooses).
-// GELU: the `act == 2` (exact erf GELU) instantiation. Kept out of the act 0 / 1 kernels: the erff expansion inside their
-// unrolled epilogue made the UNet's tc_gemm 14 % slower (same registers; one H100 80GB HBM3 at 400 W). The act 0 / 1
-// instantiations compile to the same SASS as without GELU.
-template <int BN, bool GELU, bool PP>
+// ACT: the activation compiled into the epilogue. 0: none or SiLU, chosen at run time by `act` (0 / 1); 2: exact erf GELU;
+// 3: ReLU (LPIPS's VGG16). GELU and ReLU are instantiations of their own: the erff expansion inside the unrolled act 0 / 1
+// epilogue made the UNet's tc_gemm 14 % slower (same registers; one H100 80GB HBM3 at 400 W). The ACT = 0 instantiations
+// compile to the same SASS as without GELU and ReLU.
+template <int BN, int ACT, bool PP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const TcParams p) {
     constexpr int TILE_M = PP ? 64 : 128;
@@ -351,7 +352,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     if (grow[h] < 0) continue;
                     float v0 = acc[4 * i + 2 * h] + b.x, v1 = acc[4 * i + 2 * h + 1] + b.y;
                     if (rv[h]) { v0 += rv[h][8 * i]; if (c1ok) v1 += rv[h][8 * i + 1]; }
-                    if constexpr (GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+                    if constexpr (ACT == 2) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+                    else if constexpr (ACT == 3) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
                     else if (p.act == 1) { v0 = silu(v0); v1 = silu(v1); }
                     v0 *= p.a0; v1 *= p.a0;
                     if (has1) { v0 += p.a1 * u1[h].x; if (c1ok) v1 += p.a1 * u1[h].y; }
@@ -419,11 +421,11 @@ static int num_sms_cached() {
     return n;
 }
 
-template <int BN, bool GELU, bool PP>
+template <int BN, int ACT, bool PP>
 static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, TcParams& p, cudaStream_t st) {
     static bool configured = false;
     if (!configured) {
-        GCD_CUDA_CHECK(cudaFuncSetAttribute(tc_gemm_kernel<BN, GELU, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
+        GCD_CUDA_CHECK(cudaFuncSetAttribute(tc_gemm_kernel<BN, ACT, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
         configured = true;
     }
     constexpr int STAGE_BYTES = (PP ? 64 : 128) * 128 + BN * 128;
@@ -437,7 +439,7 @@ static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, TcParams& p, 
     const int sms = num_sms_cached();
     GCD_REQUIRE(sms > 0, "tc_gemm: no CUDA device");
     const int grid = tiles < sms ? tiles : sms;
-    tc_gemm_kernel<BN, GELU, PP><<<grid, TC_THREADS, smem, st>>>(mA, mB, p);
+    tc_gemm_kernel<BN, ACT, PP><<<grid, TC_THREADS, smem, st>>>(mA, mB, p);
     GCD_CUDA_CHECK(cudaGetLastError());
     g_launches++;
     return 0;
@@ -494,7 +496,7 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
     const gcd_epilogue& e = op->ep;
     GCD_REQUIRE(!e.geglu || (op->N % 256 == 0 && !e.out_f32 && !e.res1 && !e.res2 && e.a_acc == 1.0f && !e.act),
                 "gcd_tc_run: GEGLU needs N %% 256 == 0, 16-bit output, no residual / scale / activation");
-    GCD_REQUIRE(e.act >= 0 && e.act <= 2, "gcd_tc_run: act=%d unsupported (0 none, 1 SiLU, 2 GELU)", e.act);
+    GCD_REQUIRE(e.act >= 0 && e.act <= 3, "gcd_tc_run: act=%d unsupported (0 none, 1 SiLU, 2 GELU, 3 ReLU)", e.act);
     GCD_REQUIRE(!e.rowvec || e.rows_per_vec > 0, "gcd_tc_run: rows_per_vec must be > 0");
     GCD_REQUIRE(!e.bias || ((uintptr_t)e.bias & 15) == 0, "gcd_tc_run: bias must be 16B aligned");
     GCD_REQUIRE(!e.rowvec || (((uintptr_t)e.rowvec & 15) == 0 && e.ld_rowvec % 4 == 0),
@@ -615,14 +617,15 @@ extern "C" int gcd_tc_run(const gcd_tc_op* op, void* stream) {
     tmap_cache_put(tkey, ts);
     }
     int rc;
+#define GCD_TC_LAUNCH_ACT(bn, a) (pp ? launch_tc<bn, a, true>(mA, mB, p, st) : launch_tc<bn, a, false>(mA, mB, p, st))
 #define GCD_TC_LAUNCH(bn)                                                                                  \
-    (e.act == 2 ? (pp ? launch_tc<bn, true, true>(mA, mB, p, st) : launch_tc<bn, true, false>(mA, mB, p, st)) \
-                : (pp ? launch_tc<bn, false, true>(mA, mB, p, st) : launch_tc<bn, false, false>(mA, mB, p, st)))
+    (e.act == 2 ? GCD_TC_LAUNCH_ACT(bn, 2) : e.act == 3 ? GCD_TC_LAUNCH_ACT(bn, 3) : GCD_TC_LAUNCH_ACT(bn, 0))
     switch (BN) {
         case 256: rc = GCD_TC_LAUNCH(256); break;
         case 160: rc = GCD_TC_LAUNCH(160); break;
         default: rc = GCD_TC_LAUNCH(128); break;
     }
 #undef GCD_TC_LAUNCH
+#undef GCD_TC_LAUNCH_ACT
     return rc ? rc : stats_skipped;
 }

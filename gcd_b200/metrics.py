@@ -1,5 +1,5 @@
 """Evaluation-loop metrics on the device (SURVEY.md §8(f) rank 3, first slice): per-frame PSNR / SSIM of decoded frames against
-ground truth, full-frame and over visible / occluded masks, and the per-sample aggregation of
+ground truth, full-frame and over visible / occluded masks, per-frame LPIPS (gcd_b200.lpips), and the per-sample aggregation of
 gcd-model/scripts/test.py:346-496 (`calculate_metrics`). The per-pixel work runs in ONE kernel (csrc/metrics.cu); the few
 per-frame scalars are folded on the host with the reference's own nanmean logic. No CPU fallback for the image pass."""
 import ctypes
@@ -43,10 +43,30 @@ def frame_metrics(pred, gt, mask=None):
     return res
 
 
-def calculate_metrics(gt_rgb, reproject_rgb, pred_samples_rgb):
+def frame_lpips(pred, gt, model):
+    """Per-frame LPIPS of frames in [0, 1] (validation_step, models/diffusion.py:342: `lpips(gt * 2 - 1, pred * 2 - 1)`).
+    pred: CUDA [T, 3, H, W] or [S, T, 3, H, W]; gt: CUDA [T, 3, H, W]; model: gcd_b200.lpips.LPIPS. Returns float64 CPU [T] or
+    [S, T]. With S samples the ground truth's features are computed once, not S times."""
+    if gt.dim() != 4 or pred.shape[-4:] != gt.shape or pred.dim() not in (4, 5):
+        raise ValueError(f"frame_lpips: pred {tuple(pred.shape)} does not match gt {tuple(gt.shape)} ([T,3,H,W] or [S,T,3,H,W])")
+    ops._need_cuda(pred, gt)
+    d = model.layer_distances(pred.reshape(-1, *gt.shape[1:]).float() * 2.0 - 1.0, gt.float() * 2.0 - 1.0)
+    return d.sum(0).cpu().view(pred.shape[:-3])
+
+
+def validation_metrics(gt_video, sampled_video, model):
+    """DiffusionEngine.validation_step's metrics (models/diffusion.py:317-362): the means over frames of per-frame LPIPS, PSNR and
+    SSIM. gt_video, sampled_video: CUDA float32 [frames, 3, H, W] in [0, 1]. Returns {lpips, psnr, ssim} as floats."""
+    lp = frame_lpips(sampled_video, gt_video, model)
+    m = frame_metrics(sampled_video, gt_video)
+    return {"lpips": lp.mean().item(), "psnr": m["psnr"].mean().item(), "ssim": m["ssim"].mean().item()}
+
+
+def calculate_metrics(gt_rgb, reproject_rgb, pred_samples_rgb, lpips=None):
     """gcd-model/scripts/test.py:346-496 for device tensors. gt_rgb [T,3,H,W]; reproject_rgb [T,3,H,W] or None (occluded where
     the re-projected colour is ~0, test.py:366-368); pred_samples_rgb [S,T,3,H,W]. Returns the reference's metrics dict
-    (numpy-compatible CPU tensors) with the same keys."""
+    (numpy-compatible CPU tensors) with the same keys. With an LPIPS model (gcd_b200.lpips.LPIPS) the dict also holds
+    frame_lpips (S, T) and mean_lpips (S)."""
     S = pred_samples_rgb.shape[0]
     vis = occ = None
     if reproject_rgb is not None:
@@ -68,6 +88,9 @@ def calculate_metrics(gt_rgb, reproject_rgb, pred_samples_rgb):
     unc = std.mean(dim=1)                                                   # then nanmean over channels: (T, H, W)
     out["frame_diversity"] = unc.mean(dim=(1, 2)).double().cpu()
     out["mean_diversity"] = out["frame_diversity"].mean()
+    if lpips is not None:
+        out["frame_lpips"] = frame_lpips(pred_samples_rgb, gt_rgb, lpips)
+        out["mean_lpips"] = out["frame_lpips"].mean(dim=1)
     if vis is not None:                    # test.py:470-480: the per-sample std over the masked pixels of each frame
         for name, m in (("vis", vis), ("occ", occ)):
             num = (std.double() * m[:, None]).sum(dim=(1, 2, 3))

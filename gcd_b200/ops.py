@@ -413,6 +413,48 @@ def render_views(xyz, rgb, segm, palette, desc, cams, H, W, Hp, Wp, spread_radiu
                                      int(spread_radius), _p(acc), _p(maxd), _p(out), _stream()), "render_views")
 
 
+# ------------------------------------------------------------------------------------------------ LPIPS (the GEMMs are tc_gemm ops)
+LPIPS_HEAD_PIX = 128       # GCD_LPIPS_HEAD_PIX (include/gcd_b200.h): pixels per block of gcd_lpips_head
+
+
+def lpips_input(x, shift, scale, out):
+    """x: float32 NCHW [n, 3, H, W] in [-1, 1]; shift, scale: float32 [3] (any shape of 3 contiguous values) -> out act [n*H*W, 64]:
+    the 3x3 im2col of the scaled image (columns (ky, kx, c), 0 outside the image), columns 27..63 zero."""
+    _need_cuda(x, shift, scale, out)
+    n, c, H, W = x.shape
+    assert c == 3 and x.dtype == torch.float32 and x.is_contiguous()
+    assert shift.dtype == torch.float32 and scale.dtype == torch.float32 and shift.is_contiguous() and scale.is_contiguous()
+    assert out.dtype == act_dtype() and out.shape == (n * H * W, 64) and out.is_contiguous()
+    with _timed("lpips input" if DETAIL else "lpips", 0.0, x.numel() * 4 + out.numel() * 2):
+        check(lib().gcd_lpips_input(_p(x), n, H, W, _p(shift), _p(scale), _p(out), _stream()), "lpips_input")
+
+
+def maxpool2x2(x, out):
+    """x: act [n, H, W, C] channels-last -> out act [n, H // 2, W // 2, C] (MaxPool2d(2, 2), floor mode)."""
+    _need_cuda(x, out)
+    n, H, W, C = x.shape
+    assert x.dtype == act_dtype() and x.is_contiguous() and out.is_contiguous() and out.shape == (n, H // 2, W // 2, C)
+    with _timed("lpips maxpool" if DETAIL else "lpips", 0.0, (x.numel() + out.numel()) * 2):
+        check(lib().gcd_maxpool2x2(_p(x), n, H, W, C, _p(out), _stream()), "maxpool2x2")
+
+
+def lpips_head(feat, pairs, w, partial, count, out):
+    """feat: act [frames, HW, C]; pairs: int32 [P, 2] (device) frame indices; w: float32 [C]; partial: float64 workspace of at least
+    P * ceil(HW / LPIPS_HEAD_PIX); count: int32 [>= P], zero (and left zero); out: float64 [P] <- the layer's LPIPS term of each
+    pair (spatial mean of the weighted squared difference of the unit-normalised features)."""
+    _need_cuda(feat, pairs, w, partial, count, out)
+    F_, HW, C = feat.shape
+    P = pairs.shape[0]
+    assert feat.dtype == act_dtype() and feat.is_contiguous() and w.dtype == torch.float32 and w.numel() == C and w.is_contiguous()
+    assert pairs.dtype == torch.int32 and pairs.shape == (P, 2) and pairs.is_contiguous()
+    assert partial.dtype == torch.float64 and partial.numel() >= P * ((HW + LPIPS_HEAD_PIX - 1) // LPIPS_HEAD_PIX)
+    assert count.dtype == torch.int32 and count.numel() >= P
+    assert out.dtype == torch.float64 and out.numel() == P and out.is_contiguous()
+    name = f"lpips head C{C} HW{HW}" if DETAIL else "lpips"
+    with _timed(name, 0.0, 2.0 * P * HW * C * 2):
+        check(lib().gcd_lpips_head(_p(feat), HW, C, _p(pairs), P, _p(w), _p(partial), _p(count), _p(out), _stream()), "lpips_head")
+
+
 _REPLAYED = 0
 
 

@@ -28,7 +28,8 @@ int64_t gcd_launch_count(void);
 
 /* Fused epilogue applied to every tensor-core op (rows r of the output, columns n):
  *   x      = acc[r,n] + bias[n] + rowvec[(r / rows_per_vec) * ld_rowvec + n]
- *   x      = act(x)                      (act: 0 none, 1 SiLU, 2 exact GELU 0.5 x (1 + erf(x / sqrt 2)) = nn.GELU())
+ *   x      = act(x)                      (act: 0 none, 1 SiLU, 2 exact GELU 0.5 x (1 + erf(x / sqrt 2)) = nn.GELU(),
+ *                                          3 ReLU = nn.ReLU (LPIPS's VGG16 convolutions))
  *   geglu: columns come in interleaved blocks of 16 value / 16 gate;  x = value * gelu_erf(gate)
  *          and the output has N/2 columns          (attention.py:87-94 GEGLU)
  *   out    = a_acc * x + a_res1 * res1[r,n] + a_res2 * res2[r,n]
@@ -210,6 +211,25 @@ int gcd_frame_metrics(const float* pred, const float* gt, const uint8_t* mask, i
 int gcd_render_views(const void* xyz, const uint8_t* rgb, const uint8_t* segm, const float* palette, int64_t P, int R,
                      const int32_t* desc_host, const int32_t* desc, const double* cams, int H, int W, int Hp, int Wp,
                      int spread_radius, double* acc, double* maxd, float* out, void* stream);
+
+/* LPIPS perceptual metric, VGG16 variant (gcd-model/sgm/modules/autoencoding/lpips/loss/lpips.py; DiffusionEngine.validation_step,
+ * models/diffusion.py:317-362). The 13 convolutions are gcd_tc_run ops with act = 3 (ReLU); these are the remaining stages.
+ * Input stage: in float32 NCHW [n, 3, H, W] in [-1, 1]; shift, scale: device float32 [3] (ScalingLayer: (x - shift) / scale, fp32).
+ * out: act [n*H*W, 64], row (f*H + y)*W + x: column (ky*3 + kx)*3 + c holds the scaled pixel (y + ky - 1, x + kx - 1, c), 0 outside
+ * the image (zero padding of the scaled image); columns 27..63 are 0. conv1_1 is then one 1-tap K = 64 GEMM. */
+int gcd_lpips_input(const float* in, int n, int H, int W, const float* shift, const float* scale, void* out, void* stream);
+/* MaxPool2d(2, 2), floor mode: act [n, H, W, C] channels-last -> act [n, H/2, W/2, C] (odd H or W drop the last row or column).
+ * C % 8 == 0, both tensors 16-byte aligned. */
+int gcd_maxpool2x2(const void* in, int n, int H, int W, int C, void* out, void* stream);
+/* LPIPS head of one tapped layer (relu1_2 .. relu5_3). feat: act [frames, HW, C] channels-last, C in {64, 128, 256, 512};
+ * pairs: device int32 [n_pairs, 2] frame indices (input, target); w: device float32 [C] (lin<k>.model.1.weight).
+ * out[p] = mean over the HW pixels of sum_c w[c] (a[c] / (|a| + 1e-10) - b[c] / (|b| + 1e-10))^2 with a, b the two frames'
+ * features at the pixel (norms over channels, fp32), written as float64. The reduction order is fixed: same inputs, same bits.
+ * partial: float64 [n_pairs * ceil(HW / GCD_LPIPS_HEAD_PIX)] workspace. count: uint32 [n_pairs], zero on entry; the kernel leaves
+ * it zero, so it is zeroed once when allocated. */
+#define GCD_LPIPS_HEAD_PIX 128
+int gcd_lpips_head(const void* feat, int HW, int C, const int32_t* pairs, int n_pairs, const float* w, double* partial,
+                   uint32_t* count, double* out, void* stream);
 
 #ifdef __cplusplus
 }
