@@ -83,7 +83,7 @@ attn_temporal_kernel(const act_t* __restrict__ qkv, int clips, int T, int tokens
 
 // ---------------------------------------------------------------------------------------------------------------------
 // T <= 16: one warp per (clip, position, head) on the legacy warp-level tensor path (mma.sync m16n8k16; a 14x14 problem
-// is far below tcgen05's M=64 minimum). Q/K/V rows are staged with coalesced 16-byte loads, fragments come from
+// is far below wgmma's M=64 minimum). Q/K/V rows are staged with coalesced 16-byte loads, fragments come from
 // ldmatrix, P is reused in registers as the A operand of P.V (FlashAttention-2 layout identity). HBM-bound by design.
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], const void* p) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"

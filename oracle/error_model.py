@@ -1,0 +1,83 @@
+"""Per-element error bounds of the library's kernels against float64 references, derived from the operand type.
+
+The reference of an op is computed in float64 from the same 16-bit-rounded inputs the kernel reads. Every element of the
+kernel's output y must then satisfy
+
+    |y - ref| <= u_out * |ref| + eta_out + kappa * 2^-24 * scale
+
+- u_out: unit roundoff of the stored type: 2^-11 (fp16), 2^-8 (bf16), 0 for a float32 output;
+- eta_out: half the subnormal spacing of a 16-bit stored type (2^-25 in fp16), the rounding error below its normal range;
+- scale: float64 sum of the absolute values of the terms that make up the element (|A|.|W|^T + |bias| + ... for a GEMM);
+- kappa: one constant per op class (KAPPA), the same for the fp16 and the bf16 build: both accumulate in fp32.
+
+A 16-bit fp16 output whose reference rounds past the fp16 maximum must be exactly the infinity of the reference's sign
+(IEEE round-to-nearest); within the accumulation error of the overflow threshold either outcome is accepted. bf16 has
+fp32's exponent range, so every bf16 output of these tests must be finite.
+"""
+import torch
+
+U = {torch.float16: 2.0 ** -11, torch.bfloat16: 2.0 ** -8, torch.float32: 0.0}
+ETA = {torch.float16: 2.0 ** -25, torch.bfloat16: 2.0 ** -134, torch.float32: 0.0}
+EPS32 = 2.0 ** -24                    # fp32 unit roundoff
+FP16_OVERFLOW = 65520.0               # the smallest magnitude that rounds to inf in fp16 (65504 + half an ulp)
+
+# kappa per op class, in units of 2^-24 * scale (attention: the scale carries P's 16-bit repack, see attention_scale)
+KAPPA = {
+    "gemm": 32.0,          # tc_gemm: Linear / conv / bmm with the fused epilogue (fp32 accumulation in the tensor cores)
+    "attention": 16.0,     # spatial / temporal / d80 flash attention (near one-hot rows with fp16-subnormal outputs reach ~10)
+    "norm": 32.0,          # GroupNorm / LayerNorm (fp64 or fp32 statistics, fp32 normalisation)
+    "elementwise": 8.0,    # softmax rows, CLIP preprocessing
+}
+
+
+def tol16(tol_fp16, dtype):
+    """A relative-L2 bar stated for an fp16 output, scaled to the unit roundoff of `dtype` (unchanged for fp16)."""
+    return tol_fp16 * U[dtype] / U[torch.float16]
+
+
+def gemm_scale(a, w, *terms):
+    """|a| @ |w|^T in float64 plus the absolute values of the additive epilogue terms (broadcast to the output)."""
+    s = a.double().abs() @ w.double().abs().t()
+    for t in terms:
+        s = s + t.double().abs()
+    return s
+
+
+def attention_scale(pv_abs, act_dtype):
+    """Scale of an attention output whose value sum is pv_abs = sum_j p_j |v_j|: the fp32 arithmetic, plus P rounded to the
+    16-bit operand type for the P.V MMA (u_act * sum_j p_j |v_j|, expressed in units of 2^-24)."""
+    return pv_abs * (1.0 + U[act_dtype] / EPS32)
+
+
+def check(y, ref, scale, kappa, name="", approx=None):
+    """Asserts the per-element bound for kernel output `y` against the float64 reference `ref` (same shape); `approx` adds an
+    approximation error a kernel states for itself (a polynomial activation). Returns the worst ratio of error to bound over
+    the finite elements, and prints it (pytest -s lists it per op and build)."""
+    kappa = KAPPA[kappa] if isinstance(kappa, str) else kappa
+    ref = ref.double().to(y.device)
+    scale = scale.double().to(y.device).expand_as(ref)
+    yd = y.double()
+    e_acc = kappa * EPS32 * scale
+    if approx is not None:
+        e_acc = e_acc + approx.double().to(y.device)
+    bound = U[y.dtype] * ref.abs() + ETA[y.dtype] + e_acc
+    if y.dtype == torch.float16:
+        must_inf = ref.abs() - e_acc >= FP16_OVERFLOW
+        may_inf = ref.abs() + e_acc >= FP16_OVERFLOW
+    else:
+        must_inf = may_inf = torch.zeros_like(ref, dtype=torch.bool)
+    fin = torch.isfinite(yd)
+    ok_inf = torch.isinf(yd) & may_inf & (torch.sign(yd) == torch.sign(ref))
+    err = (yd - ref).abs()
+    bad = (~fin & ~ok_inf) | (must_inf & fin) | (fin & (err > bound))
+    chk = fin & ~must_inf
+    ratio = (err[chk] / bound[chk].clamp_min(1e-300)).max().item() if chk.any() else 0.0
+    if bad.any():
+        i = bad.flatten().nonzero()[0].item()
+        idx = tuple(int(v) for v in torch.unravel_index(torch.tensor(i), ref.shape))
+        raise AssertionError(f"{name}: {int(bad.sum())} of {ref.numel()} elements outside |y - ref| <= u_out |ref| + "
+                             f"eta + {kappa:g} 2^-24 scale; first at {idx}: y {yd[idx].item():.9g}, ref {ref[idx].item():.9g}, "
+                             f"bound {bound[idx].item():.3g}, {int(must_inf.sum())} elements must overflow to inf; "
+                             f"worst error/bound {ratio:.3g}")
+    print(f"error/bound {name} [{y.dtype}]: {ratio:.3f}")
+    return ratio

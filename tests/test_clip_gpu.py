@@ -7,6 +7,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from oracle import error_model as EM
+
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")
@@ -70,15 +72,26 @@ def test_preprocess_vs_golden(ops, n, H, W):
     e = (img - ref).abs().max().item()
     print(f"preprocess {n}x{H}x{W}: max abs {e:.2e}")
     assert e <= 1e-5
+    # 16-bit patch matrix (the tower's operand type): the fp32 values, rounded
+    out16 = torch.empty(n * 257, 640, device="cuda", dtype=ops.act_dtype())
+    ops.clip_preprocess(x, taps[0] if taps else None, taps[1] if taps else None, ms, out16, scratch)
+    assert torch.equal(out16, out.to(out16.dtype))
     if (H, W) == (224, 224):                                        # pass-through: the input itself, normalised
         raw = (((x.cpu() + 1) / 2) - torch.tensor(clip.OPENAI_MEAN).view(1, 3, 1, 1)) / torch.tensor(clip.OPENAI_STD).view(1, 3, 1, 1)
         assert (unpatch(out, n, 1) - raw).abs().max().item() <= 1e-6
+        mean = torch.tensor(clip.OPENAI_MEAN, dtype=torch.float64).view(1, 3, 1, 1)
+        std = torch.tensor(clip.OPENAI_STD, dtype=torch.float64).view(1, 3, 1, 1)
+        xd = x.cpu().double()
+        ref, scale = ((xd + 1) / 2 - mean) / std, ((xd.abs() + 1) / 2 + mean) / std
+        EM.check(unpatch(out, n, 1), ref, scale, "elementwise", "clip_preprocess pass-through")
 
 
 def _attn_ref(qkv, n, L, heads):
-    q, k, v = qkv.float().view(n, L, 3, heads, 80).permute(2, 0, 3, 1, 4)
-    o = F.scaled_dot_product_attention(q, k, v)                     # fp32, scale 1/sqrt(80)
-    return o.permute(0, 2, 1, 3).reshape(n * L, heads * 80)
+    """softmax(q k^T / sqrt(80)) v in float64 and sum_j p_j |v_j|."""
+    q, k, v = qkv.double().view(n, L, 3, heads, 80).permute(2, 0, 3, 1, 4)
+    p = torch.softmax(q @ k.transpose(-1, -2) / 80 ** 0.5, -1)
+    flat = lambda o: o.permute(0, 2, 1, 3).reshape(n * L, heads * 80)
+    return flat(p @ v), flat(p @ v.abs())
 
 
 @pytest.mark.parametrize("n,L,heads,scale", [(3, 257, 16, 1.0), (2, 129, 16, 1.0), (2, 257, 4, 1.0), (1, 1024, 2, 1.0),
@@ -92,14 +105,15 @@ def test_attention_d80_vs_sdpa(ops, n, L, heads, scale):
     qkv = qkv.to(AD).cuda()
     out = torch.empty(n * L, heads * 80, device="cuda", dtype=AD)
     ops.attention_d80(qkv, n, L, heads, out)
-    ref = _attn_ref(qkv, n, L, heads)
+    ref, pv = _attn_ref(qkv, n, L, heads)
     if scale == "logit100":
         q, k, _ = qkv.float().view(n, L, 3, heads, 80).permute(2, 0, 3, 1, 4)
         mx = ((q @ k.transpose(-1, -2)) / 80 ** 0.5).abs().max().item()
         assert mx > 60, mx
     e = relerr(out, ref)
     print(f"attention_d80 n={n} L={L} heads={heads} {scale}: rel-L2 {e:.2e}")
-    assert e < 2e-3
+    assert e < EM.tol16(2e-3, AD)
+    EM.check(out, ref, EM.attention_scale(pv, AD), "attention", f"attention_d80 {n}x{L}x{heads} {scale}")
 
 
 def test_gelu_epilogue(ops):
@@ -108,16 +122,21 @@ def test_gelu_epilogue(ops):
     g = torch.Generator().manual_seed(5)
     x, w = torch.randn(M, K, generator=g).to(AD).cuda(), (torch.randn(N, K, generator=g) * K ** -0.5 * 3).to(AD).cuda()
     b = torch.randn(N, generator=g).cuda()
-    ref = F.gelu(x.float() @ w.float().t() + b)
+    acc = x.double() @ w.double().t() + b.double()
+    scale = 1.13 * EM.gemm_scale(x, w, b)                           # max |gelu'| = 1.13
+    ref = F.gelu(acc)
     out32 = torch.empty(M, N, device="cuda")
     ops.linear(x, w, ops.make_ep(out32, bias=b, act=2))
     assert relerr(out32, ref) < 2e-5
+    EM.check(out32, ref, scale, "gemm", "linear GELU fp32 out")
     out16 = torch.empty(M, N, device="cuda", dtype=AD)
     ops.linear(x, w, ops.make_ep(out16, bias=b, act=2))
-    assert relerr(out16, ref) < 1e-3
+    assert relerr(out16, ref) < EM.tol16(1e-3, AD)
+    EM.check(out16, ref, scale, "gemm", "linear GELU 16-bit out")
     # act 0 / 1 unchanged
     ops.linear(x, w, ops.make_ep(out32, bias=b, act=1))
-    assert relerr(out32, F.silu(x.float() @ w.float().t() + b)) < 2e-5
+    assert relerr(out32, F.silu(acc)) < 2e-5
+    EM.check(out32, F.silu(acc), scale, "gemm", "linear SiLU fp32 out")
 
 
 def test_layernorm_f32_with_position_add(ops):
@@ -127,8 +146,12 @@ def test_layernorm_f32_with_position_add(ops):
     gam, bet = (1 + 0.1 * torch.randn(C, generator=g)).cuda(), (0.1 * torch.randn(C, generator=g)).cuda()
     out = torch.empty(rows, C, device="cuda")
     ops.layernorm_f32(x, gam, bet, out, add=add, add_rows_per=1, add_mod=257)
-    ref = F.layer_norm(x + add.repeat(3, 1), (C,), gam, bet)
+    xs = (x + add.repeat(3, 1)).double()                            # the kernel adds in fp32 too: exact inputs of the norm
+    mean = xs.mean(-1, keepdim=True)
+    rstd = (xs.var(-1, unbiased=False, keepdim=True) + 1e-5).rsqrt()
+    ref = (xs - mean) * rstd * gam.double() + bet.double()
     assert relerr(out, ref) < 1e-6
+    EM.check(out, ref, (xs.abs() + mean.abs()) * rstd * gam.double().abs() + bet.double().abs(), "norm", "layernorm_f32")
 
 
 def _tower(tag):

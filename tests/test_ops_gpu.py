@@ -1,10 +1,16 @@
-"""GPU parity tests of the individual C-ABI ops against plain torch fp32 math on the same (16-bit rounded) inputs."""
+"""GPU parity tests of the individual C-ABI ops against float64 torch math on the same (16-bit rounded) inputs.
+
+Two checks per output: the relative L2 error over the whole tensor (bars stated for fp16 outputs, scaled to the operand type by
+EM.tol16), and the per-element bound of oracle/error_model.py, which also sees one wrong tile in a large tensor and holds the
+results beyond fp16's range to IEEE rounding (exactly +-inf in fp16, finite in bf16)."""
 import math
 import os
 
 import pytest
 import torch
 import torch.nn.functional as F
+
+from oracle import error_model as EM
 
 pytestmark = pytest.mark.gpu
 
@@ -28,6 +34,22 @@ def relerr(a, b):
     return ((a - b).norm() / (b.norm() + 1e-30)).item()
 
 
+def conv3x3_im2col(x, stride=1, pad01=False):
+    """float64 im2col of a channels-last act [n, H, W, C] for a 3x3 conv (padding 1), columns (ky, kx, c) like the packed
+    weights: [n*Ho*Wo, 9*C]."""
+    n, H, W, C = x.shape
+    xp = F.pad(x.double(), (0, 0, 1, 1, 1, 1))
+    cols = [xp[:, ky:ky + H:stride, kx:kx + W:stride, :] for ky in range(3) for kx in range(3)]
+    return torch.cat(cols, -1).reshape(-1, 9 * C)
+
+
+def conv_t3_im2col(x):
+    """float64 im2col of act [B, T, HW, C] for Conv3d (3,1,1) with padding (1,0,0), columns (kt, c): [B*T*HW, 3*C]."""
+    B, T, HW, C = x.shape
+    xp = F.pad(x.double(), (0, 0, 0, 0, 1, 1))
+    return torch.cat([xp[:, kt:kt + T] for kt in range(3)], -1).reshape(-1, 3 * C)
+
+
 @pytest.mark.parametrize("M,K,N", [(300, 320, 320), (128, 64, 1280), (1000, 1280, 192), (28, 1280, 640), (513, 960, 2560)])
 @pytest.mark.parametrize("out_f32", [True, False])
 def test_linear_plain(ops, M, K, N, out_f32):
@@ -36,8 +58,9 @@ def test_linear_plain(ops, M, K, N, out_f32):
     bias = rnd(N)
     out = torch.empty(M, N, device="cuda", dtype=torch.float32 if out_f32 else AD)
     ops.linear(x, w, ops.make_ep(out, bias=bias))
-    ref = x.float() @ w.float().t() + bias
-    assert relerr(out, ref) < (2e-5 if out_f32 else 1e-3)
+    ref = x.double() @ w.double().t() + bias.double()
+    assert relerr(out, ref) < (2e-5 if out_f32 else EM.tol16(1e-3, AD))
+    EM.check(out, ref, EM.gemm_scale(x, w, bias), "gemm", f"linear {M}x{K}x{N}")
 
 
 def test_linear_epilogue_full(ops):
@@ -49,13 +72,18 @@ def test_linear_epilogue_full(ops):
     out = torch.empty(M, N, device="cuda")
     ops.linear(x, w, ops.make_ep(out, bias=bias, rowvec=rv, rows_per_vec=100, res1=r1, a_res1=0.3, res2=r2, a_res2=0.6,
                                  a_acc=0.7, act=1))
-    acc = x.float() @ w.float().t() + bias + rv.repeat_interleave(100, 0)
-    ref = 0.7 * F.silu(acc) + 0.3 * r1 + 0.6 * r2.float()
+    rvr = rv.repeat_interleave(100, 0)
+    acc = x.double() @ w.double().t() + bias.double() + rvr.double()
+    ref = 0.7 * F.silu(acc) + 0.3 * r1.double() + 0.6 * r2.double()
     assert relerr(out, ref) < 2e-5
+    scale = 0.7 * EM.gemm_scale(x, w, bias, rvr) + 0.3 * r1.double().abs() + 0.6 * r2.double().abs()
+    EM.check(out, ref, scale, "gemm", "linear SiLU + rowvec + 2 residuals")
     # in-place residual update (out aliases res1)
     h = r1.clone()
     ops.linear(x, w, ops.make_ep(h, bias=bias, res1=h))
-    assert relerr(h, x.float() @ w.float().t() + bias + r1) < 2e-5
+    ref = x.double() @ w.double().t() + bias.double() + r1.double()
+    assert relerr(h, ref) < 2e-5
+    EM.check(h, ref, EM.gemm_scale(x, w, bias, r1), "gemm", "linear in-place residual")
 
 
 def test_linear_geglu(ops):
@@ -67,9 +95,21 @@ def test_linear_geglu(ops):
     idx = torch.arange(2 * C4).view(2, C4 // 16, 16).permute(1, 0, 2).reshape(-1).cuda()   # 16 value / 16 gate blocks
     out = torch.empty(M, C4, device="cuda", dtype=AD)
     ops.linear(x, w[idx].contiguous(), ops.make_ep(out, bias=b[idx].contiguous(), geglu=True))
-    y = x.float() @ w.float().t() + b
-    ref = y[:, :C4] * F.gelu(y[:, C4:])
-    assert relerr(out, ref) < 1.5e-3
+    ref, scale, approx = geglu_ref(x, w, b)
+    assert relerr(out, ref) < EM.tol16(1.5e-3, AD)
+    EM.check(out, ref, scale, "gemm", "linear GEGLU", approx=approx)
+
+
+def geglu_ref(x, w, b):
+    """value * gelu(gate) in float64 (w rows [0, C4) value, [C4, 2*C4) gate), its scale (the value and gate GEMM scales
+    times the sensitivities |gelu(gate)| and |value| * max |gelu'| = 1.13 |value|), and the kernel's stated approximation
+    error of the polynomial GELU (gcd_b200/csrc/common.cuh geglu: <= 1.05e-4 |v| max(|g|, 4))."""
+    C4 = w.shape[0] // 2
+    y = x.double() @ w.double().t() + b.double()
+    s = EM.gemm_scale(x, w, b)
+    v, g = y[:, :C4], y[:, C4:]
+    scale = s[:, :C4] * F.gelu(g).abs() + 1.13 * v.abs() * s[:, C4:]
+    return v * F.gelu(g), scale, 1.05e-4 * v.abs() * g.abs().clamp_min(4.0)
 
 
 def test_linear_strided_small_n(ops):
@@ -80,7 +120,9 @@ def test_linear_strided_small_n(ops):
     w = rnd(4, K, scale=K ** -0.5, dtype=AD)
     out = torch.zeros(M, 4, device="cuda")
     ops.linear(x, w, ops.make_ep(out))
-    assert relerr(out, x.float() @ w.float().t()) < 2e-5
+    ref = x.double() @ w.double().t()
+    assert relerr(out, ref) < 2e-5
+    EM.check(out, ref, EM.gemm_scale(x, w), "gemm", "linear strided N=4")
 
 
 @pytest.mark.parametrize("n,H,W,C,Co", [(3, 18, 32, 64, 128), (2, 9, 16, 128, 160), (2, 8, 128, 64, 64),
@@ -95,16 +137,16 @@ def test_conv2d_3x3(ops, n, H, W, C, Co, stride):
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
     out = torch.empty(n * Ho * Wo, Co, device="cuda")
     ops.conv2d_3x3(x, wp, ops.make_ep(out, bias=bias), stride=stride)
-    ref = F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), bias, stride=stride, padding=1)
-    ref = ref.permute(0, 2, 3, 1).reshape(n * Ho * Wo, Co)
+    a = conv3x3_im2col(x, stride)
+    ref = a @ wp.double().t() + bias.double()
     assert relerr(out, ref) < 3e-5
+    EM.check(out, ref, EM.gemm_scale(a, wp, bias), "gemm", f"conv3x3 {n}x{H}x{W}x{C}->{Co} s{stride}")
 
 
 @pytest.mark.parametrize("n,H,W,C,res,f32out", [(3, 24, 64, 448, True, True), (2, 9, 40, 640, False, False), (5, 16, 128, 960, True, True)])
 def test_conv2d_3x3_wide_tiles_n320(ops, n, H, W, C, res, f32out):
-    """N = 320 with K = 9*C >= 3840: tc_gemm mode 4 (256 x 320 pair tiles, both 160-column halves fed from one activation tile,
-    three rotating TMEM regions) incl. ragged M (phantom tiles), several passes per cluster, fp32 residual + fused GroupNorm
-    statistics and 16-bit output."""
+    """N = 320 with K = 9*C >= 3840: two 160-column tiles per row tile and long k-loops, incl. ragged M, fp32 residual +
+    fused GroupNorm statistics and 16-bit output."""
     AD = ops.act_dtype()
     Co = 320
     x = rnd(n, H, W, C, dtype=AD)
@@ -117,10 +159,14 @@ def test_conv2d_3x3_wide_tiles_n320(ops, n, H, W, C, res, f32out):
     st = torch.zeros(max(n, 64) * 64, device="cuda", dtype=torch.float64)
     ok = ops.conv2d_3x3(x, wp, ops.make_ep(out, bias=bias, res1=out if res else None, a_res1=0.5 if res else 1.0,
                                              gn_stats=(st, Co // 32, 32, H * W)))
-    ref = F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), bias, padding=1).permute(0, 2, 3, 1).reshape(rows, Co)
+    a = conv3x3_im2col(x)
+    ref = a @ wp.double().t() + bias.double()
+    scale = EM.gemm_scale(a, wp, bias)
+    del a
     if res:
-        ref = ref + 0.5 * r0
-    assert relerr(out, ref) < (3e-5 if f32out else 1e-3)
+        ref, scale = ref + 0.5 * r0.double(), scale + 0.5 * r0.double().abs()
+    assert relerr(out, ref) < (3e-5 if f32out else EM.tol16(1e-3, AD))
+    EM.check(out, ref, scale, "gemm", f"conv3x3 N=320 {n}x{H}x{W}x{C}")
     if ok:
         v = out.double().view(n, H * W, 32, Co // 32)
         want = torch.stack([v.sum((1, 3)), (v * v).sum((1, 3))], -1).reshape(-1)
@@ -136,9 +182,12 @@ def test_conv_t3(ops, B, T, HW, C, Co):
     wp = w[:, :, :, 0, 0].permute(0, 2, 1).reshape(Co, 3 * C).contiguous()
     out = torch.empty(B * T * HW, Co, device="cuda")
     ops.conv_t3(x, wp, ops.make_ep(out, bias=bias))
-    ref = F.conv3d(x.float().permute(0, 3, 1, 2).unsqueeze(-1), w.float(), bias, padding=(1, 0, 0))  # b c t hw 1
+    ref = F.conv3d(x.double().permute(0, 3, 1, 2).unsqueeze(-1), w.double(), bias.double(), padding=(1, 0, 0))  # b c t hw 1
     ref = ref.squeeze(-1).permute(0, 2, 3, 1).reshape(B * T * HW, Co)
     assert relerr(out, ref) < 3e-5
+    a = conv_t3_im2col(x)
+    assert torch.allclose(a @ wp.double().t() + bias.double(), ref)      # the im2col matches the Conv3d
+    EM.check(out, ref, EM.gemm_scale(a, wp, bias), "gemm", f"conv_t3 {B}x{T}x{HW}x{C}->{Co}")
 
 
 def test_bmm_nt(ops):
@@ -147,8 +196,10 @@ def test_bmm_nt(ops):
     a, b = rnd(G, M, K, dtype=AD), rnd(G, N, K, scale=K ** -0.5, dtype=AD)
     out = torch.empty(G * M, N, device="cuda")
     ops.bmm_nt(a, b, ops.make_ep(out))
-    ref = torch.bmm(a.float(), b.float().transpose(1, 2)).reshape(G * M, N)
+    ref = torch.bmm(a.double(), b.double().transpose(1, 2)).reshape(G * M, N)
     assert relerr(out, ref) < 2e-5
+    scale = torch.bmm(a.double().abs(), b.double().abs().transpose(1, 2)).reshape(G * M, N)
+    EM.check(out, ref, scale, "gemm", "bmm_nt")
 
 
 @pytest.mark.parametrize("n_img,rows,C,f32", [(4, 9216, 320, True), (2, 14 * 64, 640, True), (3, 100, 960, False),
@@ -163,12 +214,42 @@ def test_groupnorm(ops, n_img, rows, C, f32, silu):
     out = torch.empty(n_img * rows, C, device="cuda", dtype=AD)
     stats = torch.empty(n_img * 64, device="cuda", dtype=torch.float64)
     ops.groupnorm(x, n_img, rows, C, g, b, 1e-5, silu, out, stats)
-    xr = x.float().view(n_img, rows, C).permute(0, 2, 1)
-    ref = F.group_norm(xr, 32, g, b, 1e-5)
+    ref, scale = groupnorm_ref(x, n_img, rows, C, g, b, silu)
+    assert relerr(out, ref) < EM.tol16(1e-3, AD)
+    EM.check(out, ref, scale, "norm", f"groupnorm {n_img}x{rows}x{C} f32={f32} silu={silu}")
+
+
+def groupnorm_ref(x, n_img, rows, C, g, b, silu, groups=32):
+    """GroupNorm (+ SiLU) in float64 and its scale: the normalised magnitude |g| (|x| + |mean|) / std + |b| of each element."""
+    xr = x.double().view(n_img, rows, groups, C // groups)
+    mean = xr.mean((1, 3), keepdim=True)
+    rstd = (xr.var((1, 3), unbiased=False, keepdim=True) + 1e-5).rsqrt()
+    gg, bb = g.double().view(groups, C // groups), b.double().view(groups, C // groups)
+    ref = (xr - mean) * rstd * gg + bb
+    scale = (xr.abs() + mean.abs()) * rstd * gg.abs() + bb.abs()
     if silu:
         ref = F.silu(ref)
-    ref = ref.permute(0, 2, 1).reshape(n_img * rows, C)
-    assert relerr(out, ref) < 1e-3
+    return ref.reshape(n_img * rows, C), scale.reshape(n_img * rows, C)
+
+
+@pytest.mark.parametrize("f32", [True, False])
+def test_groupnorm_beyond_fp16_range(ops, f32):
+    """Inputs of magnitude 1e5 (16-bit inputs only where the type holds them) and a gain that takes part of the output past
+    65504: fp16 stores the IEEE-rounded +-inf there, bf16 finite values within the bound."""
+    AD = ops.act_dtype()
+    if not f32 and AD == torch.float16:
+        pytest.skip("fp16 cannot hold the 1e5 inputs")
+    n_img, rows, C = 2, 300, 320
+    x = rnd(n_img * rows, C) * 1e5 + 3e4
+    if not f32:
+        x = x.to(AD)
+    g, b = rnd(C) * 2e4 + 3e4, rnd(C) * 1e3
+    out = torch.empty(n_img * rows, C, device="cuda", dtype=AD)
+    stats = torch.empty(n_img * 64, device="cuda", dtype=torch.float64)
+    ops.groupnorm(x, n_img, rows, C, g, b, 1e-5, False, out, stats)
+    ref, scale = groupnorm_ref(x, n_img, rows, C, g, b, False)
+    assert (ref.abs() > 7e4).sum() > 100
+    EM.check(out, ref, scale, "norm", f"groupnorm |x| 1e5 f32={f32}")
 
 
 @pytest.mark.parametrize("rows,C", [(1000, 320), (77, 640), (4032, 1280)])
@@ -178,7 +259,9 @@ def test_layernorm(ops, rows, C):
     g, b = rnd(C) * 0.1 + 1, rnd(C) * 0.1
     out = torch.empty(rows, C, device="cuda", dtype=AD)
     ops.layernorm(x, g, b, out)
-    assert relerr(out, F.layer_norm(x, (C,), g, b, 1e-5)) < 1e-3
+    ref, scale = layernorm_ref(x, g, b)
+    assert relerr(out, ref) < EM.tol16(1e-3, AD)
+    EM.check(out, ref, scale, "norm", f"layernorm {rows}x{C}")
     # with frame-indexed additive embedding and sum output
     T, per = 7, 11
     add = rnd(T, C)
@@ -187,7 +270,29 @@ def test_layernorm(ops, rows, C):
     idx = (torch.arange(rows, device="cuda") // per) % T
     xs = x + add[idx]
     assert torch.equal(so, xs)
-    assert relerr(out, F.layer_norm(xs, (C,), g, b, 1e-5)) < 1e-3
+    ref, scale = layernorm_ref(xs, g, b)
+    assert relerr(out, ref) < EM.tol16(1e-3, AD)
+    EM.check(out, ref, scale, "norm", f"layernorm {rows}x{C} + frame embedding")
+
+
+def layernorm_ref(x, g, b, eps=1e-5):
+    """LayerNorm over the last dim in float64 and its scale |g| (|x| + |mean|) / std + |b|."""
+    xd = x.double()
+    mean = xd.mean(-1, keepdim=True)
+    rstd = (xd.var(-1, unbiased=False, keepdim=True) + eps).rsqrt()
+    return (xd - mean) * rstd * g.double() + b.double(), (xd.abs() + mean.abs()) * rstd * g.double().abs() + b.double().abs()
+
+
+def test_layernorm_beyond_fp16_range(ops):
+    """Inputs of magnitude 1e5 and a gain that takes part of the 16-bit output past 65504 (+-inf in fp16, finite in bf16)."""
+    rows, C = 500, 640
+    x = rnd(rows, C) * 1e5 - 2e4
+    g, b = rnd(C) * 2e4 + 3e4, rnd(C) * 1e3
+    out = torch.empty(rows, C, device="cuda", dtype=ops.act_dtype())
+    ops.layernorm(x, g, b, out)
+    ref, scale = layernorm_ref(x, g, b)
+    assert (ref.abs() > 7e4).sum() > 100
+    EM.check(out, ref, scale, "norm", "layernorm |x| 1e5")
 
 
 def test_softmax_rows(ops):
@@ -195,7 +300,10 @@ def test_softmax_rows(ops):
     x = rnd(300, 9216) * 5
     out = torch.empty(300, 9216, device="cuda", dtype=AD)
     ops.softmax_rows(x, 0.044, out)
-    assert relerr(out, torch.softmax(x * 0.044, -1)) < 2e-3
+    arg = (x.double() - x.double().amax(-1, keepdim=True)) * 0.044
+    ref = torch.softmax(arg, -1)
+    assert relerr(out, ref) < EM.tol16(2e-3, AD)
+    EM.check(out, ref, ref * (1 + arg.abs()), "elementwise", "softmax_rows")   # exp's argument carries its own rounding
 
 
 @pytest.mark.parametrize("clips,T,tokens,heads", [(2, 14, 144, 5), (1, 14, 37, 20), (1, 25, 16, 5)])
@@ -205,10 +313,12 @@ def test_attention_temporal(ops, clips, T, tokens, heads):
     qkv = rnd(clips * T, tokens, 3 * C, dtype=AD)
     out = torch.empty(clips * T, tokens, C, device="cuda", dtype=AD)
     ops.attention_temporal(qkv, clips, T, tokens, heads, out)
-    q, k, v = qkv.float().view(clips, T, tokens, 3, heads, 64).permute(3, 0, 2, 4, 1, 5)   # [clips, tokens, heads, T, 64]
-    ref = F.scaled_dot_product_attention(q, k, v)                                          # over T
-    ref = ref.permute(0, 3, 1, 2, 4).reshape(clips * T, tokens, C)
-    assert relerr(out, ref) < 2e-3
+    q, k, v = qkv.double().view(clips, T, tokens, 3, heads, 64).permute(3, 0, 2, 4, 1, 5)  # [clips, tokens, heads, T, 64]
+    p = torch.softmax(q @ k.transpose(-1, -2) * 0.125, -1)                                 # over T
+    ref = (p @ v).permute(0, 3, 1, 2, 4).reshape(clips * T, tokens, C)
+    pv = (p @ v.abs()).permute(0, 3, 1, 2, 4).reshape(clips * T, tokens, C)
+    assert relerr(out, ref) < EM.tol16(2e-3, AD)
+    EM.check(out, ref, EM.attention_scale(pv, AD), "attention", f"attention_temporal {clips}x{T}x{tokens}x{heads}")
 
 
 def test_elementwise(ops):
@@ -258,19 +368,69 @@ def test_sampler_kernels(ops):
     assert (xn - ref).abs().max() < 1e-4 * ref.abs().max()
 
 
+def test_sampler_prep_beyond_fp16_range(ops):
+    """c_in * x and the concat frames at magnitude 1e5: the IEEE-rounded 16-bit values (+-inf in fp16, finite in bf16)."""
+    AD = ops.act_dtype()
+    BT, H, W = 4, 8, 16
+    x, cc = rnd(BT, 4, H, W) * 3e5, rnd(BT, 4, H, W) * 1e5
+    c_in = 0.7
+    buf = torch.empty(2 * BT, H, W, 64, device="cuda", dtype=AD)
+    ops.sampler_prep(x, None, cc, BT, H, W, c_in, buf)
+    exact = torch.zeros(2 * BT, 64, H, W, device="cuda")                 # the fp32 arithmetic of the kernel, then rounded
+    exact[:BT, :4] = exact[BT:, :4] = x * c_in
+    exact[BT:, 4:8] = cc
+    assert torch.equal(buf, exact.permute(0, 2, 3, 1).to(AD))
+    ref = torch.zeros(2 * BT, 64, H, W, device="cuda", dtype=torch.float64)
+    ref[:BT, :4] = ref[BT:, :4] = x.double() * c_in
+    ref[BT:, 4:8] = cc.double()
+    ref = ref.permute(0, 2, 3, 1)
+    assert (ref.abs() > 7e4).sum() > 100
+    EM.check(buf, ref, ref.abs(), "elementwise", "sampler_prep |x| 1e5")
+
+
+@pytest.mark.parametrize("case", ["linear", "linear_res", "conv"])
+def test_gemm_beyond_fp16_range(ops, case):
+    """GEMM / conv results and an fp32 residual of magnitude ~1e5 stored as 16-bit: exactly +-inf where the fp16 rounding of
+    the result overflows (cooperative schedule without, ping-pong with the residual), finite values within the bound in bf16."""
+    AD = ops.act_dtype()
+    if case == "conv":
+        n, H, W, C, Co = 2, 12, 16, 64, 128
+        x = rnd(n, H, W, C, scale=300.0, dtype=AD)
+        wp = rnd(Co, 9 * C, scale=300.0 * (9 * C) ** -0.5, dtype=AD)
+        bias = rnd(Co) * 1e4
+        out = torch.empty(n * H * W, Co, device="cuda", dtype=AD)
+        ops.conv2d_3x3(x, wp, ops.make_ep(out, bias=bias))
+        a = conv3x3_im2col(x)
+        ref, scale = a @ wp.double().t() + bias.double(), EM.gemm_scale(a, wp, bias)
+    else:
+        M, K, N = 333, 256, 384
+        x, w = rnd(M, K, scale=300.0, dtype=AD), rnd(N, K, scale=300.0 * K ** -0.5, dtype=AD)
+        bias = rnd(N) * 1e4
+        out = torch.empty(M, N, device="cuda", dtype=AD)
+        r1 = rnd(M, N) * 1e5 if case == "linear_res" else None
+        ops.linear(x, w, ops.make_ep(out, bias=bias, res1=r1, a_res1=0.5))
+        ref, scale = x.double() @ w.double().t() + bias.double(), EM.gemm_scale(x, w, bias)
+        if r1 is not None:
+            ref, scale = ref + 0.5 * r1.double(), scale + 0.5 * r1.double().abs()
+    assert (ref.abs() > 7e4).sum() > 100 and (ref.abs() < 6e4).sum() > 100
+    EM.check(out, ref, scale, "gemm", f"{case} |y| ~1e5")
+
+
 def _attn_ref(qkv, frames, tokens, heads):
-    """softmax(q k^T / 8) v in fp64-accumulating fp32 torch math, chunked over queries (attention.py:332-336 semantics)."""
+    """softmax(q k^T / 8) v in float64, chunked over queries (attention.py:332-336 semantics), and sum_j p_j |v_j|."""
     C = heads * 64
-    q, k, v = qkv.float().view(frames, tokens, 3, heads, 64).permute(2, 0, 3, 1, 4)
-    outs = []
+    q, k, v = qkv.double().view(frames, tokens, 3, heads, 64).permute(2, 0, 3, 1, 4)
+    outs, pvs = [], []
     for i in range(0, tokens, 2048):
-        s = torch.matmul(q[:, :, i:i + 2048], k.transpose(-1, -2)) * 0.125
-        outs.append(torch.matmul(torch.softmax(s, -1), v))
-    return torch.cat(outs, 2).permute(0, 2, 1, 3).reshape(frames, tokens, C)
+        p = torch.softmax(torch.matmul(q[:, :, i:i + 2048], k.transpose(-1, -2)) * 0.125, -1)
+        outs.append(torch.matmul(p, v))
+        pvs.append(torch.matmul(p, v.abs()))
+    cat = lambda ts: torch.cat(ts, 2).permute(0, 2, 1, 3).reshape(frames, tokens, C)
+    return cat(outs), cat(pvs)
 
 
 # 4096 / 9216 tokens: the level-1 shape bench.py runs at latent 72x128; 4100: ragged last key block; scale 6: logits ~ +-100,
-# forces lazy rescales. (GCD_FA_EMU=4 — every 4th exponential pair on the FMA pipe — is an experiment path, off by default.)
+# the running maximum moves by large steps from key block to key block (the kernel rescales on every block).
 @pytest.mark.parametrize("frames,tokens,heads,scale", [
     (2, 256, 5, 1.5), (3, 144, 20, 1.5), (1, 576, 10, 1.5), (2, 100, 5, 1.5), (1, 2304, 5, 1.5), (2, 4, 5, 1.5),
     (2, 4096, 5, 1.5), (2, 9216, 5, 1.5), (1, 4100, 5, 1.5), (1, 9216, 5, 6.0), (1, 2304, 10, 6.0)])
@@ -280,8 +440,9 @@ def test_attention_spatial(ops, frames, tokens, heads, scale):
     qkv = rnd(frames, tokens, 3 * C, dtype=AD, scale=scale)
     out = torch.empty(frames, tokens, C, device="cuda", dtype=AD)
     ops.attention_spatial(qkv, frames, tokens, heads, out)
-    ref = _attn_ref(qkv, frames, tokens, heads)
-    assert relerr(out, ref) < 3e-3
+    ref, pv = _attn_ref(qkv, frames, tokens, heads)
+    assert relerr(out, ref) < EM.tol16(3e-3, AD)
+    EM.check(out, ref, EM.attention_scale(pv, AD), "attention", f"attention_spatial {frames}x{tokens}x{heads} scale {scale}")
 
 
 @pytest.mark.parametrize("n_img,Co,temporal", [(2, 128, False), (1, 128, True), (1, 512, False)])

@@ -1,11 +1,14 @@
 """GPU parity tests of tc_gemm's ping-pong schedule (ops with a residual or an fp32 output) at the edges of its 64-row tile geometry,
 and of the cooperative 128-row schedule (plain 16-bit output) on the same problems: tile counts that leave one
 consumer warpgroup without work or with one tile more than the other, k-step counts that do not divide the stage ring, and
-fused GroupNorm statistics whose image boundary is a 64-row but not a 128-row boundary. Same references as test_ops_gpu.py:
-plain torch fp32 math on the same (16-bit rounded) inputs."""
+fused GroupNorm statistics whose image boundary is a 64-row but not a 128-row boundary. Same references and error model as
+test_ops_gpu.py: float64 torch math on the same (16-bit rounded) inputs, the relative L2 error and the per-element bound of
+oracle/error_model.py."""
 import pytest
 import torch
 import torch.nn.functional as F
+
+from oracle import error_model as EM
 
 pytestmark = pytest.mark.gpu
 
@@ -50,8 +53,9 @@ def test_linear_tile_edges(ops, M, K, N, out_f32):
     bias = rnd(N)
     out = torch.empty(M, N, device="cuda", dtype=torch.float32 if out_f32 else AD)
     ops.linear(x, w, ops.make_ep(out, bias=bias))
-    ref = x.float() @ w.float().t() + bias
-    assert relerr(out, ref) < (2e-5 if out_f32 else 1e-3)
+    ref = x.double() @ w.double().t() + bias.double()
+    assert relerr(out, ref) < (2e-5 if out_f32 else EM.tol16(1e-3, AD))
+    EM.check(out, ref, EM.gemm_scale(x, w, bias), "gemm", f"linear {M}x{K}x{N}")
 
 
 @pytest.mark.parametrize("extra", [1, 2])
@@ -65,8 +69,10 @@ def test_linear_odd_tiles_above_sm_count(ops, extra):
     bias, r1, r2 = rnd(N), rnd(M, N), rnd(M, N, dtype=AD)
     h = r1.clone()
     ops.linear(x, w, ops.make_ep(h, bias=bias, res1=h, a_res1=0.5, res2=r2, a_res2=0.25))
-    ref = x.float() @ w.float().t() + bias + 0.5 * r1 + 0.25 * r2.float()
+    ref = x.double() @ w.double().t() + bias.double() + 0.5 * r1.double() + 0.25 * r2.double()
     assert relerr(h, ref) < 2e-5
+    scale = EM.gemm_scale(x, w, bias) + 0.5 * r1.double().abs() + 0.25 * r2.double().abs()
+    EM.check(h, ref, scale, "gemm", f"linear {tiles} tiles, 2 residuals in place")
 
 
 def test_linear_geglu_odd_tiles(ops):
@@ -78,8 +84,60 @@ def test_linear_geglu_odd_tiles(ops):
     idx = torch.arange(2 * C4).view(2, C4 // 16, 16).permute(1, 0, 2).reshape(-1).cuda()   # 16 value / 16 gate blocks
     out = torch.empty(M, C4, device="cuda", dtype=AD)
     ops.linear(x, w[idx].contiguous(), ops.make_ep(out, bias=b[idx].contiguous(), geglu=True))
-    y = x.float() @ w.float().t() + b
-    assert relerr(out, y[:, :C4] * F.gelu(y[:, C4:])) < 1.5e-3
+    ref, scale, approx = geglu_ref(x, w, b)
+    assert relerr(out, ref) < EM.tol16(1.5e-3, AD)
+    EM.check(out, ref, scale, "gemm", "linear GEGLU odd tiles", approx=approx)
+
+
+def geglu_ref(x, w, b):
+    """value * gelu(gate) in float64, its scale and the polynomial GELU's stated error (tests/test_ops_gpu.py geglu_ref)."""
+    C4 = w.shape[0] // 2
+    y = x.double() @ w.double().t() + b.double()
+    s = EM.gemm_scale(x, w, b)
+    v, g = y[:, :C4], y[:, C4:]
+    scale = s[:, :C4] * F.gelu(g).abs() + 1.13 * v.abs() * s[:, C4:]
+    return v * F.gelu(g), scale, 1.05e-4 * v.abs() * g.abs().clamp_min(4.0)
+
+
+# The last row tile holds 5 rows and the last column pair one column (N odd): the elements a wrong guard on rows or columns
+# would get wrong. Every other activation row is zero, so the rest of the output is bias (+ residuals) alone; the per-element
+# bound checks the ragged corner on its own, where a norm over the whole tensor would hide it.
+@pytest.mark.parametrize("schedule", ["cooperative", "pingpong", "geglu"])
+def test_ragged_last_tile_per_element(ops, schedule):
+    AD = ops.act_dtype()
+    K = 320
+    if schedule == "geglu":
+        M, N = 64 * 4 + 5, 512                         # 16-bit output of N / 2 columns; N % 256 == 0 is required
+    else:
+        M, N = (128 if schedule == "cooperative" else 64) * 3 + 5, 2 * 128 + 43
+    tile = 128 if schedule == "cooperative" else 64
+    r0 = (M // tile) * tile                            # first row of the ragged last row tile
+    x = rnd(M, K, dtype=AD)
+    x[:r0] = 0
+    w, b = rnd(N, K, scale=K ** -0.5, dtype=AD), rnd(N)
+    if schedule == "geglu":
+        idx = torch.arange(N).view(2, N // 32, 16).permute(1, 0, 2).reshape(-1).cuda()
+        out = torch.empty(M, N // 2, device="cuda", dtype=AD)
+        ops.linear(x, w[idx].contiguous(), ops.make_ep(out, bias=b[idx].contiguous(), geglu=True))
+        ref, scale, approx = geglu_ref(x, w, b)
+        EM.check(out[r0:], ref[r0:], scale[r0:], "gemm", "GEGLU ragged last row tile", approx=approx[r0:])
+        EM.check(out[:, -2:], ref[:, -2:], scale[:, -2:], "gemm", "GEGLU last column pair", approx=approx[:, -2:])
+        EM.check(out, ref, scale, "gemm", "GEGLU ragged", approx=approx)
+        return
+    ld = (N + 7) // 8 * 8
+    out = torch.empty(M, ld, device="cuda", dtype=AD)[:, :N]
+    ref = x.double() @ w.double().t() + b.double()
+    scale = EM.gemm_scale(x, w, b)
+    if schedule == "pingpong":                         # both residuals: 16-bit output with residuals takes the ping-pong schedule
+        r1, r2 = rnd(M, ld)[:, :N], rnd(M, ld, dtype=AD)[:, :N]
+        ops.linear(x, w, ops.make_ep(out, bias=b, res1=r1, a_res1=0.5, res2=r2, a_res2=0.25))
+        ref = ref + 0.5 * r1.double() + 0.25 * r2.double()
+        scale = scale + 0.5 * r1.double().abs() + 0.25 * r2.double().abs()
+    else:
+        ops.linear(x, w, ops.make_ep(out, bias=b))
+    EM.check(out[r0:], ref[r0:], scale[r0:], "gemm", f"{schedule} ragged last row tile")
+    EM.check(out[:, N - 1:], ref[:, N - 1:], scale[:, N - 1:], "gemm", f"{schedule} last (single) column")
+    EM.check(out, ref, scale, "gemm", f"{schedule} ragged")
 
 
 @pytest.mark.parametrize("G,M", [(3, 64), (5, 200), (7, 100)])
@@ -89,8 +147,10 @@ def test_bmm_nt_odd_batch(ops, G, M):
     a, b = rnd(G, M, K, dtype=AD), rnd(G, N, K, scale=K ** -0.5, dtype=AD)
     out = torch.empty(G * M, N, device="cuda")
     ops.bmm_nt(a, b, ops.make_ep(out))
-    ref = torch.bmm(a.float(), b.float().transpose(1, 2)).reshape(G * M, N)
+    ref = torch.bmm(a.double(), b.double().transpose(1, 2)).reshape(G * M, N)
     assert relerr(out, ref) < 2e-5
+    scale = torch.bmm(a.double().abs(), b.double().abs().transpose(1, 2)).reshape(G * M, N)
+    EM.check(out, ref, scale, "gemm", f"bmm_nt G={G} M={M}")
 
 
 @pytest.mark.parametrize("n,H,W", [(3, 3, 64), (5, 1, 64), (2, 9, 16), (3, 22, 32)])
@@ -106,9 +166,11 @@ def test_fused_groupnorm_stats_64_row_images(ops, n, H, W, out_f32):
     out = torch.empty(n * H * W, Co, device="cuda", dtype=torch.float32 if out_f32 else AD)
     st = torch.zeros(n * 64, device="cuda", dtype=torch.float64)
     produced = ops.conv2d_3x3(x, wp, ops.make_ep(out, bias=bias, gn_stats=(st, Co // 32, 32, H * W)))
-    w4 = wp.float().view(Co, 3, 3, C).permute(0, 3, 1, 2)
-    ref_out = F.conv2d(x.float().permute(0, 3, 1, 2), w4, bias, padding=1).permute(0, 2, 3, 1).reshape(n * H * W, Co)
-    assert relerr(out, ref_out) < (3e-5 if out_f32 else 1e-3)
+    w4 = wp.double().view(Co, 3, 3, C).permute(0, 3, 1, 2)
+    ref_out = F.conv2d(x.double().permute(0, 3, 1, 2), w4, bias.double(), padding=1).permute(0, 2, 3, 1).reshape(n * H * W, Co)
+    assert relerr(out, ref_out) < (3e-5 if out_f32 else EM.tol16(1e-3, AD))
+    scale = F.conv2d(x.double().abs().permute(0, 3, 1, 2), w4.abs(), bias.double().abs(), padding=1)
+    EM.check(out, ref_out, scale.permute(0, 2, 3, 1).reshape(n * H * W, Co), "gemm", f"conv3x3 {n}x{H}x{W}")
     if out_f32 and (H * W) % 64 == 0:              # fp32 output: 64-row tiles, one image per tile
         assert produced
     if produced:
