@@ -73,6 +73,8 @@ _SIGS = {
     "gcd_frame_metrics": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "gcd_render_views": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                  c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gcd_frames_prepare": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int32), c_int, c_int, c_int, c_int, c_int, c_int,
+                                    c_void_p, c_void_p, c_void_p]),
     "gcd_lpips_input": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "gcd_maxpool2x2": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "gcd_lpips_head": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

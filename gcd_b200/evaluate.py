@@ -421,22 +421,19 @@ def construct_batch(kind, traj, rgb_src, rgb_dst, reproject, fps, generator, con
 
 
 @torch.no_grad()
-def evaluate_example(hotpath, views, batch, num_samples, generator, lpips=None, decoding_t=14, num_steps=None):
-    """test.py's run_inference + calculate_metrics for one example, with all samples in one sampler run.
+def sample_example(hotpath, batch, num_samples, generator, decoding_t=14, num_steps=None):
+    """Conditions once and samples all S samples of one example as S clips of one sampler run, then decodes each clip.
 
     hotpath: a gcd_b200.pipeline.GCDHotPath with its conditioner loaded (load_clip, load_cond_encoder, and load_spherical for a
-    Kubric UNet); views: (gt, reproject), the target video and the reprojection baseline [T, 3, H, W] in [-1, 1] (batch["jpg"],
-    batch.get("reproject")); batch: construct_batch's dict; generator: the latent noise of sample s is the s-th
-    `randn([T, 4, H/8, W/8])` drawn from it, on its device (what the s-th sequential sample_video call draws from the device RNG);
-    lpips: optional gcd_b200.lpips.LPIPS (adds frame_lpips / mean_lpips to the metrics); decoding_t: frames per decoder chunk.
+    Kubric UNet); batch: a construct_batch dict; generator: the latent noise of sample s is the s-th `randn([T, 4, H/8, W/8])`
+    drawn from it, on its device (what the s-th sequential sample_video call draws from the device RNG); decoding_t: frames per
+    decoder chunk. (c, uc) are repeated S times and the S samples are S clips of one sample_latents call (test.py / infer.py call
+    sample_video S times and re-run the conditioner each time).
 
-    The conditioner runs once; (c, uc) are repeated S times and the S samples are S clips of one sample_latents call. Returns
-    (samples, metrics, uncertainty): samples a list of S dicts {cond_rgb, sampled_rgb [T, 3, H, W] in [0, 1], sampled_latent
-    [T, 4, H/8, W/8]} on the device, metrics calculate_metrics's dict (CPU tensors), uncertainty [T, H, W] on the device."""
-    from . import metrics
+    Returns (samples, sampled): samples a list of S dicts {cond_rgb, sampled_rgb [T, 3, H, W] in [0, 1], sampled_latent
+    [T, 4, H/8, W/8]}, sampled the stacked sampled_rgb [S, T, 3, H, W], all on the device."""
     if num_samples < 1:
         raise ValueError(f"num_samples must be >= 1, got {num_samples}")
-    gt, reproject = views
     dev = hotpath.device
     T = hotpath.T
     cond_frames = batch["cond_frames"].to(dev)
@@ -452,6 +449,23 @@ def evaluate_example(hotpath, views, batch, num_samples, generator, lpips=None, 
     sampled = torch.clamp((x + 1.0) / 2.0, min=0.0, max=1.0).view(num_samples, T, 3, H, W)
     cond_rgb = torch.clamp((cond_frames + 1.0) / 2.0, min=0.0, max=1.0)
     samples = [dict(cond_rgb=cond_rgb, sampled_rgb=sampled[s], sampled_latent=z[s * T:(s + 1) * T]) for s in range(num_samples)]
+    return samples, sampled
+
+
+@torch.no_grad()
+def evaluate_example(hotpath, views, batch, num_samples, generator, lpips=None, decoding_t=14, num_steps=None):
+    """test.py's run_inference + calculate_metrics for one example, with all samples in one sampler run (sample_example).
+
+    views: (gt, reproject), the target video and the reprojection baseline [T, 3, H, W] in [-1, 1] (batch["jpg"],
+    batch.get("reproject")); lpips: optional gcd_b200.lpips.LPIPS (adds frame_lpips / mean_lpips to the metrics); the other
+    arguments as sample_example's.
+
+    Returns (samples, metrics, uncertainty): samples as sample_example's, metrics calculate_metrics's dict (CPU tensors),
+    uncertainty [T, H, W] on the device."""
+    from . import metrics
+    samples, sampled = sample_example(hotpath, batch, num_samples, generator, decoding_t, num_steps)
+    gt, reproject = views
+    dev = hotpath.device
     gt01 = (gt.to(dev, torch.float32) + 1.0) / 2.0
     rep01 = None if reproject is None else (reproject.to(dev, torch.float32) + 1.0) / 2.0
     m, unc = metrics.calculate_metrics(gt01, rep01, sampled, lpips=lpips)

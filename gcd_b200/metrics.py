@@ -62,6 +62,23 @@ def validation_metrics(gt_video, sampled_video, model):
     return {"lpips": lp.mean().item(), "psnr": m["psnr"].mean().item(), "ssim": m["ssim"].mean().item()}
 
 
+def _sample_std(pred_samples_rgb):
+    return pred_samples_rgb.float().std(dim=0, unbiased=False)              # np.std(axis=0): (T, 3, H, W)
+
+
+def _diversity(std):
+    unc = std.mean(dim=1)                                                   # then nanmean over channels: (T, H, W)
+    frame_diversity = unc.mean(dim=(1, 2)).double().cpu()
+    return unc, frame_diversity, frame_diversity.mean()
+
+
+def sample_diversity(pred_samples_rgb):
+    """The spread of S samples (infer.py:185-211 calculate_metrics, test.py:458-462): pred_samples_rgb [S, T, 3, H, W] on the
+    device. Returns (uncertainty [T, H, W] on the device: the per-pixel std over samples averaged over channels, frame_diversity
+    float64 CPU [T]: its per-frame mean, mean_diversity: their mean, a float64 CPU scalar)."""
+    return _diversity(_sample_std(pred_samples_rgb))
+
+
 def calculate_metrics(gt_rgb, reproject_rgb, pred_samples_rgb, lpips=None):
     """gcd-model/scripts/test.py:346-496 for device tensors. gt_rgb [T,3,H,W]; reproject_rgb [T,3,H,W] or None (occluded where
     the re-projected colour is ~0, test.py:366-368); pred_samples_rgb [S,T,3,H,W]. Returns the reference's metrics dict
@@ -84,10 +101,8 @@ def calculate_metrics(gt_rgb, reproject_rgb, pred_samples_rgb, lpips=None):
     out = {k: torch.stack(v) for k, v in acc.items()}                     # (S, T)
     for k in keys:
         out[k.replace("frame_", "mean_")] = torch.nanmean(out[k], dim=1)  # (S)
-    std = pred_samples_rgb.float().std(dim=0, unbiased=False)               # np.std(axis=0): (T, 3, H, W)
-    unc = std.mean(dim=1)                                                   # then nanmean over channels: (T, H, W)
-    out["frame_diversity"] = unc.mean(dim=(1, 2)).double().cpu()
-    out["mean_diversity"] = out["frame_diversity"].mean()
+    std = _sample_std(pred_samples_rgb)
+    unc, out["frame_diversity"], out["mean_diversity"] = _diversity(std)
     if lpips is not None:
         out["frame_lpips"] = frame_lpips(pred_samples_rgb, gt_rgb, lpips)
         out["mean_lpips"] = out["frame_lpips"].mean(dim=1)

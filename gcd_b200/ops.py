@@ -413,6 +413,26 @@ def render_views(xyz, rgb, segm, palette, desc, cams, H, W, Hp, Wp, spread_radiu
                                      int(spread_radius), _p(acc), _p(maxd), _p(out), _stream()), "render_views")
 
 
+def frames_prepare(frames, box, out, channel_map=(0, 1, 2), out_frame=None):
+    """Decoded frames -> infer.py's input_rgb (include/gcd_b200.h gcd_frames_prepare). frames: uint8 [n, H, W, 3 | 4] (one size);
+    box: (y0, x0, ch, cw) crop box; out: float32 [frames, 3, Ho, Wo]; channel_map: input channel of output R, G, B;
+    out_frame: optional device int32 [n], the output frame of each input frame (default: frame f -> f)."""
+    _need_cuda(frames, out, out_frame)
+    n, H, W, C = frames.shape
+    assert frames.dtype == torch.uint8 and frames.is_contiguous(), "frames must be contiguous uint8 [n, H, W, C]"
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.dim() == 4 and out.shape[1] == 3
+    if out_frame is None:
+        assert out.shape[0] >= n
+    else:
+        assert out_frame.dtype == torch.int32 and out_frame.numel() == n and out_frame.is_contiguous()
+    Ho, Wo = out.shape[-2:]
+    y0, x0, ch, cw = (int(v) for v in box)
+    cmap = (ctypes.c_int32 * 3)(*[int(c) for c in channel_map])
+    with _timed("frames", 0.0, n * Ho * Wo * (4 * 3 + 3 * 4)):     # four uint8 RGB taps in, three floats out
+        check(lib().gcd_frames_prepare(_p(frames), n, H, W, C, cmap, y0, x0, ch, cw, Ho, Wo, _p(out_frame), _p(out), _stream()),
+              "frames_prepare")
+
+
 # ------------------------------------------------------------------------------------------------ LPIPS (the GEMMs are tc_gemm ops)
 LPIPS_HEAD_PIX = 128       # GCD_LPIPS_HEAD_PIX (include/gcd_b200.h): pixels per block of gcd_lpips_head
 

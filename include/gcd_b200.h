@@ -212,6 +212,18 @@ int gcd_render_views(const void* xyz, const uint8_t* rgb, const uint8_t* segm, c
                      const int32_t* desc_host, const int32_t* desc, const double* cams, int H, int W, int Hp, int Wp,
                      int spread_radius, double* acc, double* maxd, float* out, void* stream);
 
+/* Input frames of gcd-model/scripts/infer.py (sgm/data/common.py:121-199 process_image / load_video_mp4 after decoding, then
+ * infer.py:137 `(x + 1) / 2`). in: uint8 [n, H, W, C] decoded frames, C = 3 or 4 (the fourth channel is ignored); output channel c
+ * reads input channel channel_map[c] (HOST int32 [3], entries 0..2: {0, 1, 2} for RGB, {2, 1, 0} for cv2's BGR). Crop box rows
+ * [y0, y0 + ch), columns [x0, x0 + cw) (the host computes center_crop_numpy's box). p = u8 / 255 in fp32, resized from ch x cw
+ * to Ho x Wo as cv2.resize(INTER_LINEAR) does on float32 images (scale = in / out in fp64, source coordinate
+ * (d + 0.5) * scale - 0.5 rounded to fp32, floor, fraction 0 and index clamped at both borders, weights (1 - f, f) in fp32,
+ * horizontal pass then vertical, unfused fp32 products and sums); no resize when the crop already has the output size.
+ * out: float32 [frames, 3, Ho, Wo] in [0, 1], input frame f written to frame out_frame[f] (device int32 [n]) or f when out_frame is
+ * NULL; value ((p * 2 - 1) + 1) / 2 in fp32. Errors: -2 bad arguments (null pointer, sizes, crop box outside the frame, map). */
+int gcd_frames_prepare(const uint8_t* in, int n, int H, int W, int C, const int32_t* channel_map, int y0, int x0, int ch, int cw,
+                       int Ho, int Wo, const int32_t* out_frame, float* out, void* stream);
+
 /* LPIPS perceptual metric, VGG16 variant (gcd-model/sgm/modules/autoencoding/lpips/loss/lpips.py; DiffusionEngine.validation_step,
  * models/diffusion.py:317-362). The 13 convolutions are gcd_tc_run ops with act = 3 (ReLU); these are the remaining stages.
  * Input stage: in float32 NCHW [n, 3, H, W] in [-1, 1]; shift, scale: device float32 [3] (ScalingLayer: (x - shift) / scale, fp32).
