@@ -75,6 +75,7 @@ _SIGS = {
                                  c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "gcd_frames_prepare": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int32), c_int, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p, c_void_p, c_void_p]),
+    "gcd_unproject_depth": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_float, c_void_p, c_void_p]),
     "gcd_lpips_input": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "gcd_maxpool2x2": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "gcd_lpips_head": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

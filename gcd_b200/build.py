@@ -12,7 +12,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["gemm.cu", "norm.cu", "elem.cu", "attn_temporal.cu", "attn_spatial.cu", "metrics.cu", "clip.cu", "render.cu", "lpips.cu", "frames.cu"]
+SOURCES = ["gemm.cu", "norm.cu", "elem.cu", "attn_temporal.cu", "attn_spatial.cu", "metrics.cu", "clip.cu", "render.cu", "lpips.cu", "frames.cu", "unproject.cu"]
 OUT = os.path.join(HERE, "libgcd_b200.so")
 
 

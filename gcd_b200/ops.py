@@ -433,6 +433,23 @@ def frames_prepare(frames, box, out, channel_map=(0, 1, 2), out_frame=None):
               "frames_prepare")
 
 
+UNPROJECT_CLAMP, UNPROJECT_BALL_TO_PLANE = 0, 1    # GCD_UNPROJECT_* (include/gcd_b200.h)
+
+
+def unproject_depth(depth, cams, mode, out, max_depth=0.0):
+    """RGB-D unprojection of the dataset conversion (include/gcd_b200.h gcd_unproject_depth). depth: float32 [n, H, W];
+    cams: float32 [n, 16] = {fx, fy, cx, cy, R row-major, t} per image; mode: UNPROJECT_BALL_TO_PLANE (Kubric) or UNPROJECT_CLAMP
+    (ParDom, clamp to [0, max_depth]); out: fp16 [n, H*W, 3] <- world xyz."""
+    _need_cuda(depth, cams, out)
+    n, H, W = depth.shape
+    assert depth.dtype == torch.float32 and depth.is_contiguous(), "depth must be contiguous float32 [n, H, W]"
+    assert cams.dtype == torch.float32 and cams.shape == (n, 16) and cams.is_contiguous()
+    assert out.dtype == torch.float16 and out.shape == (n, H * W, 3) and out.is_contiguous()
+    with _timed("unproject", 0.0, n * H * W * (4 + 6)):     # one float32 depth in, three fp16 out per pixel
+        check(lib().gcd_unproject_depth(_p(depth), n, H, W, _p(cams), int(mode), float(max_depth), _p(out), _stream()),
+              "unproject_depth")
+
+
 # ------------------------------------------------------------------------------------------------ LPIPS (the GEMMs are tc_gemm ops)
 LPIPS_HEAD_PIX = 128       # GCD_LPIPS_HEAD_PIX (include/gcd_b200.h): pixels per block of gcd_lpips_head
 

@@ -224,6 +224,19 @@ int gcd_render_views(const void* xyz, const uint8_t* rgb, const uint8_t* segm, c
 int gcd_frames_prepare(const uint8_t* in, int n, int H, int W, int C, const int32_t* channel_map, int y0, int x0, int ch, int cw,
                        int Ho, int Wo, const int32_t* out_frame, float* out, void* stream);
 
+/* RGB-D unprojection of the dataset conversion (data-gen/data_utils.py:91-138 unproject_pixels_to_points + camera_to_world; Kubric's
+ * correct_depth_ball_plane_torch, convert_pcl_kubric.py:96-121; ParDom's clamp, convert_pcl_pardom.py:166). depth: float32 [n, H, W],
+ * one image per (frame, view). cams: device float32 [n, GCD_UNPROJECT_CAM] = {fx, fy, cx, cy (pixels), R = RT[0:3, 0:3] row-major,
+ * t = RT[0:3, 3]} as the reference builds them. mode GCD_UNPROJECT_BALL_TO_PLANE: z = depth / sqrt((tan(ax)^2 + tan(ay)^2) + 1) with
+ * the pixel's angles from torch.linspace(-fov/2, fov/2) and fov = 2 atan(rcp(2 |f|) * size); mode GCD_UNPROJECT_CLAMP:
+ * z = clamp(depth, 0, max_depth), NaN kept. x = ((u - cx) z) / fx, y = ((v - cy) z) / fy, world_i = ((R_i0 x + R_i1 y) + R_i2 z) + t_i,
+ * every operation one fp32 rounding. out: fp16 [n, H*W, 3], point v*W + u, round-to-nearest-even (overflow -> +-inf).
+ * Errors: -2 bad arguments (null pointer, n or H above 65535, unknown mode). */
+#define GCD_UNPROJECT_CAM 16
+#define GCD_UNPROJECT_CLAMP 0
+#define GCD_UNPROJECT_BALL_TO_PLANE 1
+int gcd_unproject_depth(const float* depth, int n, int H, int W, const float* cams, int mode, float max_depth, void* out, void* stream);
+
 /* LPIPS perceptual metric, VGG16 variant (gcd-model/sgm/modules/autoencoding/lpips/loss/lpips.py; DiffusionEngine.validation_step,
  * models/diffusion.py:317-362). The 13 convolutions are gcd_tc_run ops with act = 3 (ReLU); these are the remaining stages.
  * Input stage: in float32 NCHW [n, 3, H, W] in [-1, 1]; shift, scale: device float32 [3] (ScalingLayer: (x - shift) / scale, fp32).
