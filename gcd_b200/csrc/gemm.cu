@@ -152,7 +152,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     extern __shared__ __align__(1024) uint8_t smem[];     // SWIZZLE_128B tiles need 1024-byte alignment
     if ((smem_u32(smem) & 1023u) != 0) __trap();
     const int STAGES = p.stages;
-    float* sStatAll = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // [8 consumer warps][BN][sum, sum of squares]; PP: one [4][BN][2] half per warpgroup
+    double* sStatAll = reinterpret_cast<double*>(smem + STAGES * STAGE_BYTES);  // [8 consumer warps][BN][sum, sum of squares]; PP: one [4][BN][2] half per warpgroup
     uint64_t* bars = reinterpret_cast<uint64_t*>(sStatAll + (p.gn_stats ? 8 * BN * 2 : 0));
     uint64_t* full = bars;                 // [STAGES]
     uint64_t* empty = bars + 8;            // [STAGES]  (STAGES <= 8)
@@ -217,7 +217,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     const int st_t = PP ? (threadIdx.x & 127) : threadIdx.x - 128;
     const int st_w = PP ? (warp & 3) : warp - 4;
     const int st_bar = PP ? 1 + cw : 1;
-    float* sStat = sStatAll + (PP ? cw * (4 * BN * 2) : 0);
+    double* sStat = sStatAll + (PP ? cw * (4 * BN * 2) : 0);
     // GroupNorm statistics: party thread g < gn_groups owns group g of the party's current image and flushes it
     // (fp64 atomics) when its tile stream moves to another image — tiles of one image are many, the atomics per image few.
     int cur_img = -1;
@@ -343,7 +343,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             const bool c0ok = col < p.N, c1ok = col + 1 < p.N;
             float2 u1[2] = {t1[0], t1[1]}, u2[2] = {t2[0], t2[1]};
             if (i + 1 < BN / 8) load_res(i + 1, t1, t2);
-            float s1a = 0.f, s2a = 0.f, s1b = 0.f, s2b = 0.f;   // statistics of columns col, col + 1 over this thread's rows
+            // statistics of columns col, col + 1 over this thread's rows, in fp64 up to the global sums: the consumer's variance
+            // is sum(v^2)/n - mean^2, which fp32 partials cancel for columns whose mean is large against their spread
+            double s1a = 0.0, s2a = 0.0, s1b = 0.0, s2b = 0.0;
             if (c0ok) {
                 float2 b = make_float2(0.f, 0.f);
                 if (bias) b = c1ok ? __ldg(reinterpret_cast<const float2*>(bias + 8 * i)) : make_float2(__ldg(bias + 8 * i), 0.f);
@@ -369,8 +371,11 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                         const float2 r = unpack2(w);             // statistics of the stored (rounded) values
                         v0 = r.x; v1 = r.y;
                     }
-                    s1a += v0; s2a += v0 * v0;
-                    if (c1ok) { s1b += v1; s2b += v1 * v1; }
+                    if (stats) {                            // fp64 conversions only where statistics are requested
+                        const double d0 = v0, d1 = v1;      // exact squares of fp32 values
+                        s1a += d0; s2a += d0 * d0;
+                        if (c1ok) { s1b += d1; s2b += d1 * d1; }
+                    }
                 }
             }
             if (stats) {                            // fold the 8 row-groups of the warp (lanes with equal lane % 4)
@@ -380,7 +385,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     s1b += __shfl_xor_sync(0xffffffffu, s1b, off); s2b += __shfl_xor_sync(0xffffffffu, s2b, off);
                 }
                 if (lane < 4) {
-                    float* d = sStat + (st_w * BN + 8 * i + cb) * 2;
+                    double* d = sStat + (st_w * BN + 8 * i + cb) * 2;
                     d[0] = s1a; d[1] = s2a; d[2] = s1b; d[3] = s2b;
                 }
             }
@@ -390,7 +395,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             // The barrier spans the statistics party only: under PP the other warpgroup is in its main loop.
             named_bar_sync(st_bar, ST_THREADS);
             for (int c = st_t; c < BN; c += ST_THREADS) {
-                float a = 0.f, b = 0.f;
+                double a = 0.0, b = 0.0;
 #pragma unroll
                 for (int w = 0; w < ST_WARPS; w++) { a += sStat[(w * BN + c) * 2]; b += sStat[(w * BN + c) * 2 + 1]; }
                 sStat[c * 2] = a; sStat[c * 2 + 1] = b;
@@ -401,7 +406,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             if (img != cur_img) { flush(); cur_img = img; }
             if (st_t < p.gn_groups) {
                 const int lo = max(st_t * p.gn_cpg, n0), hi = min(min((st_t + 1) * p.gn_cpg, n0 + BN), p.N);
-                for (int c = lo; c < hi; c++) { st1 += (double)sStat[(c - n0) * 2]; st2 += (double)sStat[(c - n0) * 2 + 1]; }
+                for (int c = lo; c < hi; c++) { st1 += sStat[(c - n0) * 2]; st2 += sStat[(c - n0) * 2 + 1]; }
             }
             named_bar_sync(st_bar, ST_THREADS);     // sStat is rewritten by the next tile
         }
@@ -429,7 +434,7 @@ static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, TcParams& p, 
         configured = true;
     }
     constexpr int STAGE_BYTES = (PP ? 64 : 128) * 128 + BN * 128;
-    const int fixed = (p.gn_stats ? 8 * BN * 2 * 4 : 0) + TC_BAR_BYTES;     // statistics tables + barriers
+    const int fixed = (p.gn_stats ? 8 * BN * 2 * 8 : 0) + TC_BAR_BYTES;     // fp64 statistics tables + barriers
     int stages = (TC_SMEM_MAX - fixed) / STAGE_BYTES;
     if (stages > 8) stages = 8;
     GCD_REQUIRE(stages >= 2, "tc_gemm: not enough shared memory for the pipeline (BN=%d)", BN);

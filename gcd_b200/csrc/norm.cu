@@ -11,19 +11,43 @@ extern std::atomic<int64_t> g_launches;
 // ---------------------------------------------------------------------------------------------- GroupNorm stats
 // grid: (row_chunks, n_img). block: (C/4, RY). Each thread owns 4 consecutive channels = 2 channel pairs
 // (a pair never straddles a group because C/groups is even).
+//
+// Accuracy: the consumer derives var = sum(x^2)/n - mean^2, whose two terms are both about mean^2, so the sums are kept in
+// fp64 from each element on (fp32 partials lost the difference for groups whose mean is large against their spread:
+// |mean|/std = 1e3 cost ~1e-2 of rstd). The square of an fp32 value is exact in fp64.
+// Determinism (no floating-point smem atomics: run-to-run bit differences in the statistics flipped 16-bit roundings
+// downstream): per-thread partials -> smem [RY][C/2 pairs] -> one thread per group folds its pairs in a fixed order -> one
+// fp64 atomic per (block, group) and moment. Before the atomic, each block rounds its two sums to multiples of 2^-26 rms and
+// 2^-26 rms^2 (rms of the block's group values, rounded down to a power of two), so blocks of similar rms add values on a
+// common grid, exactly and in any order, while the rounding stays far below the accuracy the consumer needs.
+__device__ __forceinline__ void gn_block_stats(const double* sm, int npairs, int cpg, int groups, int64_t nrows,
+                                               double* __restrict__ st) {
+    const int tid = threadIdx.y * blockDim.x + threadIdx.x;
+    if (tid >= groups) return;
+    const int ppg = cpg >> 1;                          // channel pairs per group
+    double s = 0.0, q = 0.0;
+    for (int y = 0; y < (int)blockDim.y; y++) {
+        const double* row = sm + ((size_t)y * npairs + (size_t)tid * ppg) * 2;
+        for (int pp = 0; pp < ppg; pp++) { s += row[2 * pp]; q += row[2 * pp + 1]; }
+    }
+    if (q > 0.0 && q <= 1e300) {
+        const int e = ilogb(q / ((double)nrows * cpg)) >> 1;     // ~log2(rms)
+        s = ldexp(rint(ldexp(s, 26 - e)), e - 26);
+        q = ldexp(rint(ldexp(q, 26 - 2 * e)), 2 * e - 26);
+    }
+    atomicAdd(&st[tid * 2 + 0], s);
+    atomicAdd(&st[tid * 2 + 1], q);
+}
+
 template <bool IN_F32>
 __global__ void gn_stats_kernel(const void* __restrict__ in, int64_t rows, int C, int cpg, int rows_per_block,
                                 double* __restrict__ stats, int groups) {
-    // Deterministic block reduction (no floating-point smem atomics: run-to-run bit differences in the statistics
-    // flipped 16-bit roundings downstream): per-thread fp32 partials -> smem [RY][C/2 pairs] -> one thread per group
-    // folds its pairs in a fixed order in fp64 -> one fp64 atomic per (block, group).
-    extern __shared__ float sm[];                      // [blockDim.y][C/2][2]
-    const int tid = threadIdx.y * blockDim.x + threadIdx.x;
+    extern __shared__ double sm[];                     // [blockDim.y][C/2][2]
     const int img = blockIdx.y;
     const int c = threadIdx.x * 4;
     const int64_t r0 = (int64_t)blockIdx.x * rows_per_block;
     const int64_t r1 = min(rows, r0 + rows_per_block);
-    float sa = 0.f, qa = 0.f, sb = 0.f, qb = 0.f;
+    double sa = 0.0, qa = 0.0, sb = 0.0, qb = 0.0;
 #pragma unroll 4
     for (int64_t r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
         const int64_t off = ((int64_t)img * rows + r) * C + c;
@@ -36,28 +60,20 @@ __global__ void gn_stats_kernel(const void* __restrict__ in, int64_t rows, int C
             float2 a = unpack2(v.x), b = unpack2(v.y);
             x0 = a.x; x1 = a.y; x2 = b.x; x3 = b.y;
         }
-        sa += x0 + x1; qa += x0 * x0 + x1 * x1;
-        sb += x2 + x3; qb += x2 * x2 + x3 * x3;
+        const double d0 = x0, d1 = x1, d2 = x2, d3 = x3;
+        sa += d0 + d1; qa += d0 * d0 + d1 * d1;
+        sb += d2 + d3; qb += d2 * d2 + d3 * d3;
     }
     const int npairs = C >> 1;
-    float* mine = sm + ((size_t)threadIdx.y * npairs + 2 * threadIdx.x) * 2;
+    double* mine = sm + ((size_t)threadIdx.y * npairs + 2 * threadIdx.x) * 2;
     mine[0] = sa; mine[1] = qa; mine[2] = sb; mine[3] = qb;
     __syncthreads();
-    if (tid < groups) {
-        const int ppg = cpg >> 1;                      // channel pairs per group
-        double s = 0.0, q = 0.0;
-        for (int y = 0; y < (int)blockDim.y; y++) {
-            const float* row = sm + ((size_t)y * npairs + (size_t)tid * ppg) * 2;
-            for (int pp = 0; pp < ppg; pp++) { s += (double)row[2 * pp]; q += (double)row[2 * pp + 1]; }
-        }
-        atomicAdd(&stats[((int64_t)img * groups + tid) * 2 + 0], s);
-        atomicAdd(&stats[((int64_t)img * groups + tid) * 2 + 1], q);
-    }
+    gn_block_stats(sm, npairs, cpg, groups, r1 - r0, stats + (int64_t)img * groups * 2);
 }
 
 // Channel concat of two fp32 tensors fused with the GroupNorm statistics of the result (the UNet's skip concatenations,
 // openaimodel.py `th.cat([h, hs.pop()], dim=1)` followed by the ResBlock's first GroupNorm): same geometry and the same
-// deterministic reduction as gn_stats_kernel; saves the statistics pass over the concatenated tensor.
+// deterministic fp64 reduction as gn_stats_kernel; saves the statistics pass over the concatenated tensor.
 // OUT_ACT: the concatenated tensor is written in the 16-bit activation type only — the consumer ResBlock always has
 // cin != cout there (its 1x1 skip conv and its first GroupNorm read 16-bit operands; nothing reads the fp32 concat), which removes
 // the fp32 write of the concat, the fp32 read of the GroupNorm and the separate cast pass: 20 -> 10 bytes per element.
@@ -66,8 +82,7 @@ template <bool OUT_ACT>
 __global__ void concat_stats_kernel(const float* __restrict__ a, int Ca, const float* __restrict__ b, int Cb, int64_t rows,
                                     int cpg, int rows_per_block, void* __restrict__ out_, double* __restrict__ stats,
                                     int groups) {
-    extern __shared__ float sm[];                      // [blockDim.y][C/2][2]
-    const int tid = threadIdx.y * blockDim.x + threadIdx.x;
+    extern __shared__ double sm[];                     // [blockDim.y][C/2][2]
     const int img = blockIdx.y;
     const int C = Ca + Cb;
     const int c = threadIdx.x * 4;
@@ -76,30 +91,22 @@ __global__ void concat_stats_kernel(const float* __restrict__ a, int Ca, const f
     const int ld = from_a ? Ca : Cb;
     const int64_t r0 = (int64_t)blockIdx.x * rows_per_block;
     const int64_t r1 = min(rows, r0 + rows_per_block);
-    float sa = 0.f, qa = 0.f, sb = 0.f, qb = 0.f;
+    double sa = 0.0, qa = 0.0, sb = 0.0, qb = 0.0;
 #pragma unroll 4
     for (int64_t r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
         const int64_t row = (int64_t)img * rows + r;
         const float4 v = *reinterpret_cast<const float4*>(src + row * ld);
         if (OUT_ACT) *reinterpret_cast<uint2*>(reinterpret_cast<act_t*>(out_) + row * C + c) = make_uint2(pack2(v.x, v.y), pack2(v.z, v.w));
         else *reinterpret_cast<float4*>(reinterpret_cast<float*>(out_) + row * C + c) = v;
-        sa += v.x + v.y; qa += v.x * v.x + v.y * v.y;
-        sb += v.z + v.w; qb += v.z * v.z + v.w * v.w;
+        const double d0 = v.x, d1 = v.y, d2 = v.z, d3 = v.w;
+        sa += d0 + d1; qa += d0 * d0 + d1 * d1;
+        sb += d2 + d3; qb += d2 * d2 + d3 * d3;
     }
     const int npairs = C >> 1;
-    float* mine = sm + ((size_t)threadIdx.y * npairs + 2 * threadIdx.x) * 2;
+    double* mine = sm + ((size_t)threadIdx.y * npairs + 2 * threadIdx.x) * 2;
     mine[0] = sa; mine[1] = qa; mine[2] = sb; mine[3] = qb;
     __syncthreads();
-    if (tid < groups) {
-        const int ppg = cpg >> 1;
-        double s = 0.0, q = 0.0;
-        for (int y = 0; y < (int)blockDim.y; y++) {
-            const float* row = sm + ((size_t)y * npairs + (size_t)tid * ppg) * 2;
-            for (int pp = 0; pp < ppg; pp++) { s += (double)row[2 * pp]; q += (double)row[2 * pp + 1]; }
-        }
-        atomicAdd(&stats[((int64_t)img * groups + tid) * 2 + 0], s);
-        atomicAdd(&stats[((int64_t)img * groups + tid) * 2 + 1], q);
-    }
+    gn_block_stats(sm, npairs, cpg, groups, r1 - r0, stats + (int64_t)img * groups * 2);
 }
 
 template <bool IN_F32>
@@ -179,7 +186,7 @@ extern "C" int gcd_groupnorm_stats(const void* in, int in_f32, int64_t n_img, in
     int rc = gn_geometry(n_img, rows, C, groups, &grid, &block, &rpb);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t smem = (size_t)block.y * (C / 2) * 2 * sizeof(float);
+    const size_t smem = (size_t)block.y * (C / 2) * 2 * sizeof(double);
     GCD_REQUIRE(smem <= 48 * 1024 && (int)(block.x * block.y) >= groups, "groupnorm_stats: unsupported geometry (C=%d)", C);
     if (in_f32)
         gn_stats_kernel<true><<<grid, block, smem, st>>>(in, rows, C, C / groups, rpb, stats, groups);
@@ -198,7 +205,7 @@ extern "C" int gcd_concat_channels_stats(const float* a, int Ca, const float* b,
     const int C = Ca + Cb;
     int rc = gn_geometry(n_img, rows, C, groups, &grid, &block, &rpb);
     if (rc) return rc;
-    const size_t smem = (size_t)block.y * (C / 2) * 2 * sizeof(float);
+    const size_t smem = (size_t)block.y * (C / 2) * 2 * sizeof(double);
     GCD_REQUIRE(smem <= 48 * 1024 && (int)(block.x * block.y) >= groups, "concat_stats: unsupported geometry (C=%d)", C);
     concat_stats_kernel<false><<<grid, block, smem, (cudaStream_t)stream>>>(a, Ca, b, Cb, rows, C / groups, rpb, out, stats, groups);
     GCD_CUDA_CHECK(cudaGetLastError());
@@ -214,7 +221,7 @@ extern "C" int gcd_concat_channels_stats_act(const float* a, int Ca, const float
     const int C = Ca + Cb;
     int rc = gn_geometry(n_img, rows, C, groups, &grid, &block, &rpb);
     if (rc) return rc;
-    const size_t smem = (size_t)block.y * (C / 2) * 2 * sizeof(float);
+    const size_t smem = (size_t)block.y * (C / 2) * 2 * sizeof(double);
     GCD_REQUIRE(smem <= 48 * 1024 && (int)(block.x * block.y) >= groups, "concat_stats_act: unsupported geometry (C=%d)", C);
     concat_stats_kernel<true><<<grid, block, smem, (cudaStream_t)stream>>>(a, Ca, b, Cb, rows, C / groups, rpb, out, stats, groups);
     GCD_CUDA_CHECK(cudaGetLastError());
@@ -331,11 +338,17 @@ layernorm_rows_kernel(const float* __restrict__ in, int64_t rows, const float* _
                 const float2* ad = reinterpret_cast<const float2*>(add + ((row / add_rows_per) % add_mod) * C);
 #pragma unroll
                 for (int k = 0; k < NK; k++) { float2 a = __ldg(&ad[lane + 32 * k]); v[r][k].x += a.x; v[r][k].y += a.y; }
-                if (sum_out) {
-                    float2* so = reinterpret_cast<float2*>(sum_out + row * C);
+            }
+        }
+    }
+    if (sum_out) {                                     // in (+ add), like the generic kernel: also written without `add`
 #pragma unroll
-                    for (int k = 0; k < NK; k++) so[lane + 32 * k] = v[r][k];
-                }
+        for (int r = 0; r < ROWS; r++) {
+            const int64_t row = row0 + r;
+            if (row < rows) {
+                float2* so = reinterpret_cast<float2*>(sum_out + row * C);
+#pragma unroll
+                for (int k = 0; k < NK; k++) so[lane + 32 * k] = v[r][k];
             }
         }
     }

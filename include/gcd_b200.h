@@ -89,7 +89,9 @@ int gcd_tc_run(const gcd_tc_op* op, void* stream);
 /* ---- normalisation (HBM-bound kernels) ------------------------------------------------------------------ */
 /* GroupNorm statistics over `rows_per_group_img` rows x (C/groups) channels: util.py:274-276 GroupNorm32,
  * attention.py:125-128 Normalize. in: [n_img*rows, C] float32 (in_f32=1) or act. stats: double[n_img*groups*2]
- * (sum, sumsq), must be zeroed by the caller (gcd_memset_async) before the call. */
+ * (sum, sumsq), must be zeroed by the caller (gcd_memset_async) before the call. The sums are accumulated in fp64 from
+ * each element on, so the variance gcd_groupnorm_apply derives from them (sumsq/n - mean^2) holds for groups whose mean
+ * is large against their spread. */
 int gcd_groupnorm_stats(const void* in, int in_f32, int64_t n_img, int64_t rows, int C, int groups, double* stats,
                         void* stream);
 /* y = (x-mean)*rstd*gamma+beta, optional SiLU, written as act. */
@@ -98,7 +100,8 @@ int gcd_groupnorm_apply(const void* in, int in_f32, int64_t n_img, int64_t rows,
                         void* stream);
 /* LayerNorm over C per row (attention.py BasicTransformerBlock norm1-3, video_attention.py norm_in/1/2/3).
  * in: float32 [rows, C]. Optional `add` [n_add, C] float32 is added first with index (row / add_rows_per) % add_mod
- * (video_attention.py:266-287 time_pos_embed) and the sum written to sum_out (float32) when non-NULL. */
+ * (video_attention.py:266-287 time_pos_embed). When sum_out is non-NULL, the tensor that is normalised (in + add, or in
+ * alone without `add`) is written to it as float32, for every C. */
 int gcd_layernorm(const float* in, int64_t rows, int C, const float* gamma, const float* beta, float eps,
                   const float* add, int64_t add_rows_per, int64_t add_mod, float* sum_out, void* out, void* stream);
 /* The same LayerNorm (with the same optional `add`) written as float32 [rows, C]: open_clip VisionTransformer's ln_pre, whose

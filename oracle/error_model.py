@@ -25,7 +25,7 @@ FP16_OVERFLOW = 65520.0               # the smallest magnitude that rounds to in
 KAPPA = {
     "gemm": 32.0,          # tc_gemm: Linear / conv / bmm with the fused epilogue (fp32 accumulation in the tensor cores)
     "attention": 16.0,     # spatial / temporal / d80 flash attention (near one-hot rows with fp16-subnormal outputs reach ~10)
-    "norm": 32.0,          # GroupNorm / LayerNorm (fp64 or fp32 statistics, fp32 normalisation)
+    "norm": 32.0,          # GroupNorm (fp64 sums from each element on) / LayerNorm (two-pass fp32), fp32 normalisation
     "elementwise": 8.0,    # softmax rows, CLIP preprocessing
 }
 

@@ -281,7 +281,9 @@ def _cfg_worker(rank, world, port, q):
     import torch.distributed as dist
     dist.init_process_group("gloo", init_method=f"tcp://127.0.0.1:{port}", rank=rank, world_size=world)
     out = _cfg_run(dist.new_group([0, 1]))
-    q.put((rank, out))
+    # by value: a tensor put on a torch.multiprocessing queue is passed as a shared-memory handle that the receiver fetches
+    # from this process, which may already have exited by then (EOFError in the receiver)
+    q.put((rank, out.numpy()))
     dist.destroy_process_group()
 
 
@@ -294,7 +296,7 @@ def test_cfg_parallel_world2_gloo_equals_single_process():
     port = 30100 + os.getpid() % 500
     ps = [ctx.Process(target=_cfg_worker, args=(r, 2, port, q)) for r in range(2)]
     [p.start() for p in ps]
-    res = dict(q.get(timeout=120) for _ in ps)
+    res = {r: torch.from_numpy(a) for r, a in (q.get(timeout=120) for _ in ps)}
     [p.join(timeout=60) for p in ps]
     assert torch.equal(res[0], res[1])
     assert torch.allclose(res[0], ref, rtol=0, atol=1e-6)

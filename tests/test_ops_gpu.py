@@ -202,8 +202,11 @@ def test_bmm_nt(ops):
     EM.check(out, ref, scale, "gemm", "bmm_nt")
 
 
-@pytest.mark.parametrize("n_img,rows,C,f32", [(4, 9216, 320, True), (2, 14 * 64, 640, True), (3, 100, 960, False),
-                                              (2, 333, 128, True), (1, 50, 2560, True), (2, 77, 512, False)])
+GN_SHAPES = [(4, 9216, 320, True), (2, 14 * 64, 640, True), (3, 100, 960, False), (2, 333, 128, True), (1, 50, 2560, True),
+             (2, 77, 512, False)]
+
+
+@pytest.mark.parametrize("n_img,rows,C,f32", GN_SHAPES)
 @pytest.mark.parametrize("silu", [False, True])
 def test_groupnorm(ops, n_img, rows, C, f32, silu):
     AD = ops.act_dtype()
@@ -230,6 +233,122 @@ def groupnorm_ref(x, n_img, rows, C, g, b, silu, groups=32):
     if silu:
         ref = F.silu(ref)
     return ref.reshape(n_img * rows, C), scale.reshape(n_img * rows, C)
+
+
+# ---- GroupNorm on groups whose mean is large against their spread. GroupNorm derives the variance as sum(x^2)/n - mean^2
+# from the (sum, sum of squares) its producers accumulate: both terms are about mean^2, so the sums must be accurate far
+# beyond fp32 for the difference to be. The reference (GroupNorm32: F.group_norm on x.float(), Welford moments) has no such
+# limit. Inputs: R + sigma z per group, with a per-channel spread of +-1 % of sigma.
+def offset_tensor(rows, C, R, sigma, dtype=torch.float32, seed=[0]):
+    """[rows, C] = R + sigma * z + (+-1 % of sigma per channel), generated on the device, in `dtype`."""
+    seed[0] += 1
+    g = torch.Generator(device="cuda").manual_seed(seed[0])
+    x = torch.randn(rows, C, device="cuda", generator=g).mul_(sigma)
+    x.add_(R + 0.01 * sigma * (2 * torch.rand(C, device="cuda", generator=g) - 1))
+    return x if dtype == torch.float32 else x.to(dtype)
+
+
+def large_mean_16(dtype):
+    """(R, sigma) for a 16-bit tensor: R = 3e4 (the fp16 range holds R + 5 sigma) and sigma = 8 ulps at R, so the spread
+    survives the rounding. |mean| / std is then ~234 in fp16 and ~29 in bf16."""
+    R = 3e4
+    return R, 8 * 2.0 ** (math.floor(math.log2(R)) - (10 if dtype == torch.float16 else 7))
+
+
+def group_moments(x, n_img, rows, C, groups=32):
+    """float64 mean and variance (two-pass, centred) per (image, group) of x [n_img*rows, C], in row chunks (a float64
+    copy of the largest tensors would not fit)."""
+    xv = x.view(n_img, rows, groups, C // groups)
+    step = max(1, (1 << 24) // (n_img * C))
+    s = torch.zeros(n_img, groups, dtype=torch.float64, device=x.device)
+    for r in range(0, rows, step):
+        s += xv[:, r:r + step].double().sum((1, 3))
+    mean = s / (rows * (C // groups))
+    q = torch.zeros_like(s)
+    for r in range(0, rows, step):
+        q += (xv[:, r:r + step].double() - mean[:, None, :, None]).square().sum((1, 3))
+    return mean, q / (rows * (C // groups))
+
+
+def check_group_stats(st, x, n_img, rows, C, name, groups=32):
+    """The mean and variance GroupNorm derives from the statistics buffer (sum, sum of squares per (image, group); the
+    variance as gcd_groupnorm_apply forms it) against float64 moments of x, the tensor the producer read or stored:
+        |d mean| <= 2^-19 (|mean| + std),   |d var| <= 2^-18 std (|mean| + std),
+    linear in |mean| / std like the per-element bound of the "norm" class (oracle/error_model.py). Prints both worst
+    error/bound ratios and returns the float64 moments and |mean| / std per group."""
+    mean, var = group_moments(x, n_img, rows, C, groups)
+    cnt = rows * (C // groups)
+    s = st[: n_img * groups * 2].view(n_img, groups, 2)
+    km = s[..., 0] / cnt
+    kv = s[..., 1] / cnt - km * km
+    std = var.sqrt()
+    rm = ((km - mean).abs() / (2.0 ** -19 * (mean.abs() + std))).max().item()
+    rv = ((kv - var).abs() / (2.0 ** -18 * std * (mean.abs() + std))).max().item()
+    print(f"error/bound {name} statistics: mean {rm:.3f}, variance {rv:.3f}")
+    assert rm <= 1 and rv <= 1, f"{name}: statistics error/bound mean {rm:.3g}, variance {rv:.3g}"
+    return mean, var, mean.abs() / std
+
+
+def groupnorm_ref_rows(x, idx, rows, mean, var, g, b, silu, groups=32):
+    """groupnorm_ref for the rows `idx` of x [n_img*rows, C], from float64 moments of the whole tensor."""
+    C = x.shape[1]
+    xr = x[idx].double().view(len(idx), groups, C // groups)
+    img = idx // rows
+    m, rstd = mean[img][:, :, None], (var[img][:, :, None] + 1e-5).rsqrt()
+    gg, bb = g.double().view(groups, C // groups), b.double().view(groups, C // groups)
+    ref = (xr - m) * rstd * gg + bb
+    scale = (xr.abs() + m.abs()) * rstd * gg.abs() + bb.abs()
+    if silu:
+        ref = F.silu(ref)
+    return ref.reshape(len(idx), C), scale.reshape(len(idx), C)
+
+
+@pytest.mark.parametrize("n_img,rows,C", [s[:3] for s in GN_SHAPES])
+@pytest.mark.parametrize("R", [1e2, 1e3, 1e4, "16-bit"])
+def test_groupnorm_large_mean(ops, n_img, rows, C, R):
+    """gcd_groupnorm_stats + apply on groups with |mean| / std = R (float32 input, std 1) or the largest a 16-bit input
+    holds: the statistics, then the output with its own statistics pass and, with SiLU, from the same statistics."""
+    AD = ops.act_dtype()
+    (R, sigma), dt = (large_mean_16(AD), AD) if R == "16-bit" else ((R, 1.0), torch.float32)
+    x = offset_tensor(n_img * rows, C, R, sigma, dt)
+    g, b = rnd(C) * 0.1 + 1, rnd(C) * 0.1
+    out = torch.empty(n_img * rows, C, device="cuda", dtype=AD)
+    stats = torch.empty(n_img * 64, device="cuda", dtype=torch.float64)
+    name = f"groupnorm {n_img}x{rows}x{C} {dt} R={R:g}"
+    ops.groupnorm(x, n_img, rows, C, g, b, 1e-5, False, out, stats)
+    _, _, ratio = check_group_stats(stats, x, n_img, rows, C, name)
+    assert ratio.min() > 0.5 * R / sigma, ratio.min()
+    ref, scale = groupnorm_ref(x, n_img, rows, C, g, b, False)
+    EM.check(out, ref, scale, "norm", name)
+    ops.groupnorm(x, n_img, rows, C, g, b, 1e-5, True, out, stats, have_stats=True)
+    ref, scale = groupnorm_ref(x, n_img, rows, C, g, b, True)
+    EM.check(out, ref, scale, "norm", name + " SiLU")
+
+
+# The GroupNorm statistics images of the production forward, which give the statistics kernel the most rows per thread.
+@pytest.mark.parametrize("n_img,rows,C", [(28, 9216, 320),            # UNet spatial GroupNorm (14 frames x CFG)
+                                          (2, 14 * 9216, 320),        # UNet temporal: one image per clip of 14 frames
+                                          (1, 14 * 576 * 1024, 128)])  # VAE decoder temporal GroupNorm at full resolution
+@pytest.mark.parametrize("f32", [True, False])
+def test_groupnorm_large_mean_production_images(ops, n_img, rows, C, f32):
+    """Statistics over every row against float64; the outputs (without and with SiLU) on a strided sample of rows."""
+    AD = ops.act_dtype()
+    (R, sigma), dt = ((1e4, 1.0), torch.float32) if f32 else (large_mean_16(AD), AD)
+    x = offset_tensor(n_img * rows, C, R, sigma, dt)
+    g, b = rnd(C) * 0.1 + 1, rnd(C) * 0.1
+    out = torch.empty(n_img * rows, C, device="cuda", dtype=AD)
+    stats = torch.empty(n_img * 64, device="cuda", dtype=torch.float64)
+    name = f"groupnorm {n_img}x{rows}x{C} {dt} R={R:g}"
+    ops.groupnorm(x, n_img, rows, C, g, b, 1e-5, False, out, stats)
+    mean, var, ratio = check_group_stats(stats, x, n_img, rows, C, name)
+    assert ratio.min() > 0.5 * R / sigma, ratio.min()
+    idx = torch.cat([torch.arange(0, n_img * rows, n_img * rows // 16384 + 1, device="cuda"),
+                     torch.tensor([n_img * rows - 1], device="cuda")])
+    ref, scale = groupnorm_ref_rows(x, idx, rows, mean, var, g, b, False)
+    EM.check(out[idx], ref, scale, "norm", name + " (row sample)")
+    ops.groupnorm(x, n_img, rows, C, g, b, 1e-5, True, out, stats, have_stats=True)
+    ref, scale = groupnorm_ref_rows(x, idx, rows, mean, var, g, b, True)
+    EM.check(out[idx], ref, scale, "norm", name + " SiLU (row sample)")
 
 
 @pytest.mark.parametrize("f32", [True, False])
@@ -281,6 +400,26 @@ def layernorm_ref(x, g, b, eps=1e-5):
     mean = xd.mean(-1, keepdim=True)
     rstd = (xd.var(-1, unbiased=False, keepdim=True) + eps).rsqrt()
     return (xd - mean) * rstd * g.double() + b.double(), (xd.abs() + mean.abs()) * rstd * g.double().abs() + b.double().abs()
+
+
+@pytest.mark.parametrize("C", [320, 640, 1280, 192, 512])
+def test_layernorm_large_mean(ops, C):
+    """Rows with |mean| / std = 1e4 (a control: LayerNorm is two-pass in fp32) through the specialised C = 320 / 640 / 1280
+    kernels and the generic one, 16-bit and float32 outputs. `sum_out` without `add` receives the input itself."""
+    rows = 1000
+    x = offset_tensor(rows, C, 1e4, 1.0)
+    xd = x.double()
+    assert (xd.mean(-1).abs() / xd.std(-1, unbiased=False)).min() > 5e3
+    g, b = rnd(C) * 0.1 + 1, rnd(C) * 0.1
+    out = torch.empty(rows, C, device="cuda", dtype=ops.act_dtype())
+    so = torch.full_like(x, float("nan"))
+    ops.layernorm(x, g, b, out, sum_out=so)
+    assert torch.equal(so, x)
+    ref, scale = layernorm_ref(x, g, b)
+    EM.check(out, ref, scale, "norm", f"layernorm {rows}x{C} R=1e4")
+    out32 = torch.empty(rows, C, device="cuda")
+    ops.layernorm_f32(x, g, b, out32)
+    EM.check(out32, ref, scale, "norm", f"layernorm_f32 {rows}x{C} R=1e4")
 
 
 def test_layernorm_beyond_fp16_range(ops):
@@ -553,3 +692,31 @@ def test_concat_channels_with_fused_groupnorm_stats(ops, n, rows, Ca, Cb):
     st3 = torch.zeros_like(st)
     ops.concat_channels(a, b, out16, stats=st3, n_img=n)
     assert torch.equal(out16, ref.to(AD)) and torch.equal(st3, st)
+
+
+@pytest.mark.parametrize("n,rows,Ca,Cb", [(3, 100, 64, 192), (28, 144, 1280, 1280), (2, 9216, 640, 320)])
+@pytest.mark.parametrize("where", ["a", "b", "both"])
+@pytest.mark.parametrize("R", [1e2, 1e3, 1e4])
+def test_concat_channels_large_mean(ops, n, rows, Ca, Cb, where, R):
+    """gcd_concat_channels_stats[_act] with the offset R (std 1) in `a`, in `b` or in both: the statistics against float64
+    over the concatenation, equal in both variants, and the GroupNorm (without and with SiLU) that consumes them."""
+    C = Ca + Cb
+    a = offset_tensor(n * rows, Ca, R if where != "b" else 0.0, 1.0)
+    b = offset_tensor(n * rows, Cb, R if where != "a" else 0.0, 1.0)
+    out = torch.empty(n * rows, C, device="cuda")
+    st = torch.zeros(n * 64, device="cuda", dtype=torch.float64)
+    ops.concat_channels(a, b, out, stats=st, n_img=n)
+    assert torch.equal(out, torch.cat([a, b], 1))
+    name = f"concat_stats {n}x{rows}x({Ca}+{Cb}) offset in {where} R={R:g}"
+    _, _, ratio = check_group_stats(st, out, n, rows, C, name)
+    assert ratio.max() > 0.5 * R, ratio.max()
+    AD = ops.act_dtype()
+    st16 = torch.zeros_like(st)
+    ops.concat_channels(a, b, torch.empty(n * rows, C, device="cuda", dtype=AD), stats=st16, n_img=n)
+    assert torch.equal(st16, st)                      # the 16-bit variant sums the same fp32 inputs in the same order
+    g, be = rnd(C) * 0.1 + 1, rnd(C) * 0.1
+    y = torch.empty(n * rows, C, device="cuda", dtype=AD)
+    for silu in (False, True):
+        ops.groupnorm(out, n, rows, C, g, be, 1e-5, silu, y, st, have_stats=True)
+        ref, scale = groupnorm_ref(out, n, rows, C, g, be, silu)
+        EM.check(y, ref, scale, "norm", name + (" SiLU" if silu else ""))

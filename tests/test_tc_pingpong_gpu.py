@@ -9,6 +9,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import error_model as EM
+from test_ops_gpu import check_group_stats, groupnorm_ref, large_mean_16, offset_tensor
 
 pytestmark = pytest.mark.gpu
 
@@ -177,3 +178,58 @@ def test_fused_groupnorm_stats_64_row_images(ops, n, H, W, out_f32):
         v = out.double().view(n, H * W, 32, Co // 32)
         ref = torch.stack([v.sum((1, 3)), (v * v).sum((1, 3))], -1).reshape(-1)
         assert torch.allclose(st, ref, rtol=1e-5, atol=1e-3)
+
+
+# Fused GroupNorm statistics of outputs whose groups have a mean R times their spread, the offset planted through the bias,
+# through res1 or through a per-image row vector (the time-embedding row of the UNet ResBlock's first conv). A 16-bit output
+# without a residual runs the cooperative schedule, an fp32 output or one with a residual the ping-pong schedule. Shapes: the
+# 64-row images above (ping-pong only: a 128-row tile cannot keep them apart), one image per 128-row tile, and the per-CTA
+# accumulation shapes of test_ops_gpu.py::test_fused_groupnorm_stats_accumulated (conv 3x3 and Conv3d (3,1,1)).
+def _large_mean_cases():
+    cases = []
+    for n, H, W, Co, temporal, pp_only, Rs in [(3, 3, 64, 320, False, True, (1e2, 1e3, 1e4)),
+                                               (5, 1, 64, 320, False, True, (1e2, 1e3, 1e4)),
+                                               (3, 22, 32, 320, False, True, (1e2, 1e3, 1e4)),
+                                               (3, 8, 128, 320, False, False, (1e2, 1e3, 1e4)),
+                                               (2, 192, 512, 128, False, False, (1e4,)),
+                                               (4, 1, 48 * 512, 128, True, False, (1e4,))]:
+        for plant in ("bias", "res1", "rowvec"):
+            for R in Rs:                                   # float32 output: ping-pong
+                cases.append((n, H, W, Co, temporal, plant, R))
+            if plant == "res1" or not pp_only:             # 16-bit output: ping-pong with res1, else cooperative
+                cases.append((n, H, W, Co, temporal, plant, "16-bit"))
+    return cases
+
+
+@pytest.mark.parametrize("n,H,W,Co,temporal,plant,R", _large_mean_cases())
+def test_fused_groupnorm_stats_large_mean(ops, n, H, W, Co, temporal, plant, R):
+    AD = ops.act_dtype()
+    out_f32 = R != "16-bit"
+    R, sigma = (R, 1.0) if out_f32 else large_mean_16(AD)
+    C, rpi = 64, H * W
+    if temporal:                                   # Conv3d (3,1,1) over [B=1, T=n, H*W, C]; statistics over the whole clip
+        x = rnd(1, n, H * W, C, dtype=AD)
+        wp = rnd(Co, 3 * C, scale=sigma * (3 * C) ** -0.5, dtype=AD)
+        n, rpi = 1, n * H * W
+        run = lambda ep: ops.conv_t3(x, wp, ep)
+    else:
+        x = rnd(n, H, W, C, dtype=AD)
+        wp = rnd(Co, 9 * C, scale=sigma * (9 * C) ** -0.5, dtype=AD)
+        run = lambda ep: ops.conv2d_3x3(x, wp, ep)
+    rows = n * rpi
+    offset = offset_tensor(n, Co, R, 0.005 * sigma)  # per image and channel: R + ~1 % of sigma
+    bias = offset[0].contiguous() if plant == "bias" else rnd(Co, scale=0.01 * sigma)
+    res1 = offset.repeat_interleave(rpi, 0) if plant == "res1" else None
+    rowvec = offset if plant == "rowvec" else None
+    out = torch.empty(rows, Co, device="cuda", dtype=torch.float32 if out_f32 else AD)
+    st = torch.zeros(n * 64, device="cuda", dtype=torch.float64)
+    assert run(ops.make_ep(out, bias=bias, rowvec=rowvec, rows_per_vec=rpi, res1=res1, gn_stats=(st, Co // 32, 32, rpi)))
+    name = f"fused statistics {'t3' if temporal else 'conv3x3'} {rows}x{Co} {out.dtype} offset in {plant} R={R:g}"
+    _, _, ratio = check_group_stats(st, out, n, rpi, Co, name)
+    assert ratio.min() > 0.5 * R / sigma, ratio.min()
+    g, b = rnd(Co) * 0.1 + 1, rnd(Co) * 0.1
+    y = torch.empty(rows, Co, device="cuda", dtype=AD)
+    for silu in (False, True):
+        ops.groupnorm(out, n, rpi, Co, g, b, 1e-5, silu, y, st, have_stats=True)
+        ref, scale = groupnorm_ref(out, n, rpi, Co, g, b, silu)
+        EM.check(y, ref, scale, "norm", name + (" SiLU" if silu else ""))
