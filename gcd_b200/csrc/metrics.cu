@@ -3,16 +3,30 @@
 // scikit-image 0.22.0 `structural_similarity(data_range=1, channel_axis=0)` and gcd-model/scripts/eval_utils.py:571-664
 // (masked_ssim: the same map averaged over an eroded mask): 7x7 uniform window, sample covariance (NP/(NP-1)), K1 = 0.01,
 // K2 = 0.03, the 3-pixel border strip ignored, mean over the three channels.
-// HBM-bound streaming work (2 x 4 B per pixel-channel read once; 10 MB per 576x1024 frame pair): one block per 32x16 output tile,
-// the 38x22 halo of both images staged in shared memory, every thread sums its own 7x7 window (fp32, like the float32 images
-// of the reference), block reduction in fp64, one fp64 atomic per block and quantity.
+// One block per 32x16 output tile and channel, the 38x22 halo of both images staged in shared memory. The arithmetic follows the
+// reference's float32 numpy / scipy arithmetic, because in flat and near-flat windows (sky, floors, 8-bit levels) SSIM is the
+// difference of two nearly equal window means over C2 = 9e-4, and any other rounding of those means moves it by up to 1e-3:
+//   * products x*x, y*y, x*y rounded to fp32;
+//   * window means as scipy.ndimage.uniform_filter forms them: a vertical pass (axis 0) then a horizontal one, each summing its
+//     7 fp32 inputs in fp64, dividing by 7 in fp64 and rounding to fp32 once (the vertical means of the tile's 38 halo columns
+//     go through a shared-memory table); scipy keeps a running mean instead of a fresh sum, which rarely lands one fp32 ulp away;
+//   * the SSIM formula in fp32 in numpy's operation order, every operation rounded on its own (no FMA contraction);
+//   * PSNR: the difference squared in fp32 (skimage's mean_squared_error on float32 images), summed in fp64.
+// Block reduction in fp64, one fp64 atomic per block and quantity.
 #include "common.cuh"
 #include "../../include/gcd_b200.h"
 #include <atomic>
 extern std::atomic<int64_t> g_launches;
 
 namespace {
-constexpr int TX = 32, TY = 16, R = 3, HX = TX + 2 * R, HY = TY + 2 * R;
+constexpr int TX = 32, TY = 16, R = 3, HX = TX + 2 * R, HY = TY + 2 * R, NQ = 5;
+
+// s / 7 correctly rounded in fp64 (Markstein: q0 = s * RN(1/7) is within one ulp and the remainder s - 7 q0 is exact), then
+// rounded to fp32: one pass of scipy's uniform_filter1d on a float32 array
+__device__ __forceinline__ float mean7(double s) {
+    const double q0 = __dmul_rn(s, 1.0 / 7.0);
+    return __double2float_rn(__fma_rn(__fma_rn(-7.0, q0, s), 1.0 / 7.0, q0));
+}
 
 // out per frame: [0] sum sq. diff (all), [1] count, [2] sum sq. diff (mask), [3] count (mask), [4] sum SSIM (cropped map),
 // [5] count, [6] sum SSIM over the eroded mask, [7] count  — sums over the 3 channels
@@ -21,6 +35,7 @@ frame_metrics_kernel(const float* __restrict__ a, const float* __restrict__ b, c
                      double* __restrict__ out) {
     __shared__ float sa[HY][HX + 1], sb[HY][HX + 1];
     __shared__ uint8_t sm[HY][HX + 1];
+    __shared__ double vmean[NQ][TY][HX];       // vertical 7-row means (fp32 values) of x, y, x*x, y*y, x*y per halo column
     __shared__ double red[8][TX * TY / 32];
     const int f = blockIdx.z / 3, c = blockIdx.z % 3;
     const float* pa = a + ((int64_t)f * 3 + c) * H * W;
@@ -35,26 +50,47 @@ frame_metrics_kernel(const float* __restrict__ a, const float* __restrict__ b, c
         sm[ly][lx] = (in && pm) ? pm[(int64_t)y * W + x] : 0;      // binary_erosion border_value = 0
     }
     __syncthreads();
+    if (threadIdx.x < 2 * NQ * HX) {           // vertical pass: one thread per quantity, halo column and half of the tile's rows
+        const int q = threadIdx.x / (2 * HX), lx = threadIdx.x % HX, r0 = (threadIdx.x / HX) % 2 * (TY / 2);
+        double v[TY / 2 + 2 * R];
+#pragma unroll
+        for (int r = 0; r < TY / 2 + 2 * R; r++) {   // quantity q = u * w with u, w in {x, y, 1} (x * 1 is exact)
+            const float x = sa[r0 + r][lx], y = sb[r0 + r][lx];
+            const float u = (q == 1 || q == 3) ? y : x, w = q < 2 ? 1.f : (q == 2 ? x : y);
+            v[r] = (double)__fmul_rn(u, w);
+        }
+#pragma unroll
+        for (int r = 0; r < TY / 2; r++) {
+            double s = v[r];
+#pragma unroll
+            for (int k = 1; k < 7; k++) s += v[r + k];
+            vmean[q][r0 + r][lx] = (double)mean7(s);
+        }
+    }
+    __syncthreads();
     const int lx = threadIdx.x % TX, ly = threadIdx.x / TX, x = x0 + lx, y = y0 + ly;
     double v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     if (x < W && y < H) {
-        const float d = sa[ly + R][lx + R] - sb[ly + R][lx + R];
-        v[0] = (double)d * d; v[1] = 1.0;
+        const float d = __fsub_rn(sa[ly + R][lx + R], sb[ly + R][lx + R]);
+        v[0] = (double)__fmul_rn(d, d); v[1] = 1.0;
         if (pm && sm[ly + R][lx + R]) { v[2] = v[0]; v[3] = 1.0; }
         if (x >= R && x < W - R && y >= R && y < H - R) {          // crop(S, pad): windows fully inside the image
-            float ux = 0.f, uy = 0.f, uxx = 0.f, uyy = 0.f, uxy = 0.f;
+            float m[NQ];                                            // ux, uy, uxx, uyy, uxy
 #pragma unroll
-            for (int dy = 0; dy < 7; dy++)
+            for (int q = 0; q < NQ; q++) {                          // horizontal pass over the 7 vertical means
+                double s = vmean[q][ly][lx];
 #pragma unroll
-                for (int dx = 0; dx < 7; dx++) {
-                    const float p = sa[ly + dy][lx + dx], q = sb[ly + dy][lx + dx];
-                    ux += p; uy += q; uxx += p * p; uyy += q * q; uxy += p * q;
-                }
-            const float inv = 1.0f / 49.0f, cov = 49.0f / 48.0f;
-            ux *= inv; uy *= inv; uxx *= inv; uyy *= inv; uxy *= inv;
-            const float vx = cov * (uxx - ux * ux), vy = cov * (uyy - uy * uy), vxy = cov * (uxy - ux * uy);
-            const float C1 = 1e-4f, C2 = 9e-4f;
-            const float S = ((2.f * ux * uy + C1) * (2.f * vxy + C2)) / ((ux * ux + uy * uy + C1) * (vx + vy + C2));
+                for (int k = 1; k < 7; k++) s += vmean[q][ly][lx + k];
+                m[q] = mean7(s);
+            }
+            const float ux = m[0], uy = m[1], uxx = m[2], uyy = m[3], uxy = m[4];
+            const float cov = (float)(49.0 / 48.0), C1 = (float)(0.01 * 0.01), C2 = (float)(0.03 * 0.03);
+            const float ux2 = __fmul_rn(ux, ux), uy2 = __fmul_rn(uy, uy);
+            const float vx = __fmul_rn(cov, __fsub_rn(uxx, ux2)), vy = __fmul_rn(cov, __fsub_rn(uyy, uy2)),
+                        vxy = __fmul_rn(cov, __fsub_rn(uxy, __fmul_rn(ux, uy)));
+            const float A1 = __fadd_rn(__fmul_rn(__fmul_rn(2.f, ux), uy), C1), A2 = __fadd_rn(__fmul_rn(2.f, vxy), C2);
+            const float B1 = __fadd_rn(__fadd_rn(ux2, uy2), C1), B2 = __fadd_rn(__fadd_rn(vx, vy), C2);
+            const float S = __fdiv_rn(__fmul_rn(A1, A2), __fmul_rn(B1, B2));
             v[4] = S; v[5] = 1.0;
             if (pm) {          // binary_erosion(mask, iterations = 3) with the cross element = all pixels within L1 distance 3
                 bool ok = true;

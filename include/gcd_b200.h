@@ -196,7 +196,10 @@ void gcd_tc_override(int bn, int mode);
  * structural_similarity(data_range=1, channel_axis=0), masked form = gcd-model/scripts/eval_utils.py:571-664 masked_ssim).
  * pred, gt: float32 [frames, 3, H, W] in [0, 1]; mask: uint8 [frames, H, W] or NULL. out: float64 [frames, 8], zeroed here:
  *   {sum (pred-gt)^2, count, same over mask, count, sum SSIM map (3-pixel border cropped), count, same over the 3x eroded mask, count},
- * sums over the 3 channels. PSNR = 10 log10(count / sum) for data_range 1; SSIM = sum / count. */
+ * sums over the 3 channels. PSNR = 10 log10(count / sum) for data_range 1; SSIM = sum / count.
+ * The per-pixel arithmetic is the reference's float32 arithmetic: (pred-gt)^2 squared in fp32; window means as scipy's
+ * uniform_filter forms them (fp32 products, a vertical then a horizontal 7-tap pass, each summed in fp64 and rounded to fp32
+ * once); the SSIM formula in fp32 in numpy's order without FMA contraction. Identical images give SSIM exactly 1. */
 int gcd_frame_metrics(const float* pred, const float* gt, const uint8_t* mask, int frames, int H, int W, double* out, void* stream);
 
 /* Point-cloud view synthesis of the evaluation clips (gcd-model/sgm/data/geometry.py:242-444 project_points_to_pixels +

@@ -1,5 +1,6 @@
 """Pins oracle/metrics_oracle.py to the REFERENCE's own `masked_ssim` (gcd-model/scripts/eval_utils.py:571-664), executed in the
-build container, and writes tests/golden/metrics.pt (TEST INFRASTRUCTURE; needs /root/reference).
+build container, and writes tests/golden/metrics.pt (smoothed noise) and tests/golden/metrics_flat.pt (flat, near-flat and 8-bit
+frames at 72 x 104 plus a batch of 7 x 7 frames with one SSIM window each) (TEST INFRASTRUCTURE; needs the reference checkout).
 
 `masked_ssim` imports four helpers from scikit-image (0.22.0 in the reference's requirements_versions.txt, not installed here):
 `_supported_float_type`, `check_shape_equality`, `slice_at_axis`, `crop` — one-liners provided below as a stub `skimage` package;
@@ -62,3 +63,37 @@ if __name__ == "__main__":
         out["ssim_all"].append(float(r[0])); out["ssim_masked"].append(float(r[1])); out["psnr"].append(float(M.psnr(pred[t].numpy(), gt[t].numpy())))
     torch.save(out, os.path.join(ROOT, "tests", "golden", "metrics.pt"))
     print("[metrics] oracle == reference masked_ssim (both results) on", T, "frames:", out["ssim_all"], out["ssim_masked"], out["psnr"])
+
+    # flat and near-flat content, where SSIM is most sensitive to how the window means are rounded
+    H, W = 72, 104
+    lv = torch.tensor([0.93, 0.41, 0.17])[:, None, None]
+    step = torch.tensor([1.0, -1.0, 1.0])[:, None, None] / 255
+    flat = lv.expand(3, H, W).clone()
+    near = lv + 1e-3 * torch.randn(3, H, W, generator=g)
+    b8 = torch.randint(0, 256, (3, (H + 31) // 32, (W + 31) // 32), generator=g).float() / 255
+    b8 = b8.repeat_interleave(32, 1).repeat_interleave(32, 2)[:, :H, :W]
+    gt = torch.stack([flat, near, b8]).float()
+    pred = torch.stack([flat + step, lv + 1e-3 * torch.randn(3, H, W, generator=g),
+                        b8 + torch.randint(-1, 2, (3, H, W), generator=g) / 255]).clamp(0, 1).float()
+    mask = torch.zeros(3, H, W, dtype=torch.bool)
+    mask[0, :, :52] = True; mask[1, 8:64, 16:96] = True; mask[1, 30:34, 40:44] = False; mask[2] = torch.rand(H, W, generator=g) > 0.05
+    # 7 x 7 frames: one window per channel (flat 8-bit levels +- 1/255, level + 1e-3 noise, random 8-bit levels)
+    N = 64
+    lev = torch.randint(0, 256, (N, 3, 1, 1), generator=g).float() / 255
+    g7 = torch.cat([lev[:24].expand(24, 3, 7, 7), lev[24:48] + 1e-3 * torch.randn(24, 3, 7, 7, generator=g),
+                    torch.randint(0, 256, (16, 3, 7, 7), generator=g).float() / 255]).clamp(0, 1).float()
+    p7 = torch.cat([g7[:24] + torch.where(torch.rand(24, 3, 1, 1, generator=g) < 0.5, 1.0, -1.0) / 255,
+                    lev[24:48] + 1e-3 * torch.randn(24, 3, 7, 7, generator=g),
+                    g7[48:] + torch.randint(-1, 2, (16, 3, 7, 7), generator=g) / 255]).clamp(0, 1).float()
+    m7 = torch.rand(N, 7, 7, generator=g) > 0.05
+    flat_out = {"gt": gt, "pred": pred, "mask": mask, "gt7": g7, "pred7": p7, "mask7": m7}
+    for key, (P, G, Mk) in (("", (pred, gt, mask)), ("7", (p7, g7, m7))):
+        rows = [(f(P[t].numpy(), G[t].numpy(), Mk[t].numpy()), M.ssim_pair(P[t].numpy(), G[t].numpy(), Mk[t].numpy()))
+                for t in range(P.shape[0])]
+        for r, o in rows:
+            assert abs(r[0] - o[0]) < 1e-12 and (abs(r[1] - o[1]) < 1e-12 or (np.isnan(r[1]) and np.isnan(o[1]))), (r, o)
+        flat_out["ssim_all" + key] = [float(r[0]) for r, _ in rows]
+        flat_out["ssim_masked" + key] = [float(r[1]) for r, _ in rows]
+    torch.save(flat_out, os.path.join(ROOT, "tests", "golden", "metrics_flat.pt"))
+    print("[metrics] oracle == reference masked_ssim on 3 flat / near-flat / 8-bit frames and", N, "one-window frames:",
+          flat_out["ssim_all"], flat_out["ssim_masked"])
