@@ -10,6 +10,18 @@ kernel's output y must then satisfy
 - scale: float64 sum of the absolute values of the terms that make up the element (|A|.|W|^T + |bias| + ... for a GEMM);
 - kappa: one constant per op class (KAPPA), the same for the fp16 and the bf16 build: both accumulate in fp32.
 
+tc_gemm's k-loop adds a one-sided term. Each wgmma k16 step adds 16 products to the fp32 accumulator and rounds toward zero,
+so every step loses a little of the running sum P_i (the exact sum after step i), always toward zero. Measured on one H100
+80GB HBM3 with all-positive operands, the loss is 2.4-3.8 * 2^-24 |P_i| per step on average over the outputs, and about 4.4
+at worst. For zero-mean operands P_i random-walks around zero and these losses stay within kappa. For same-sign
+operands P_i grows through the k-loop, and the error grows linearly with K: -1.75 (K / 16) 2^-24 sum |a||w| on average when
+the running sum grows evenly (1.5e-4 of the result at K = 23040). The bound of a GEMM whose test computes the running sums adds
+
+    GEMM_STEP * 2^-24 * steps,    steps = sum_i |P_i| <= ceil(K / 16) * scale    (gemm_step_sums)
+
+GEMM_STEP = 8 allows four truncations of under one fp32 ulp (2^-23 |P_i|) per k16 step, about twice the measured worst case.
+Tests that leave `steps` out hold the kernel to kappa alone; they use zero-mean operands.
+
 A 16-bit fp16 output whose reference rounds past the fp16 maximum must be exactly the infinity of the reference's sign
 (IEEE round-to-nearest); within the accumulation error of the overflow threshold either outcome is accepted. bf16 has
 fp32's exponent range, so every bf16 output of these tests must be finite.
@@ -28,6 +40,7 @@ KAPPA = {
     "norm": 32.0,          # GroupNorm (fp64 sums from each element on) / LayerNorm (two-pass fp32), fp32 normalisation
     "elementwise": 8.0,    # softmax rows, CLIP preprocessing
 }
+GEMM_STEP = 8.0            # tc_gemm: round-toward-zero loss per wgmma k16 step, in units of 2^-24 * |running sum|
 
 
 def tol16(tol_fp16, dtype):
@@ -43,21 +56,37 @@ def gemm_scale(a, w, *terms):
     return s
 
 
+def gemm_step_sums(a, w, step=16):
+    """sum over the k-steps of tc_gemm's k-loop of |running sum of a . w| in float64, per output element: a [..., M, K],
+    w [..., N, K] with columns in the kernel's k order (the packed (tap, channel) order of a convolution's im2col)."""
+    a, w = a.double(), w.double().transpose(-1, -2)
+    K = a.shape[-1]
+    run = torch.zeros(a.shape[:-1] + w.shape[-1:], dtype=torch.float64, device=a.device)
+    total = torch.zeros_like(run)
+    for k0 in range(0, K, step):
+        run += a[..., k0:k0 + step] @ w[..., k0:k0 + step, :]
+        total += run.abs()
+    return total
+
+
 def attention_scale(pv_abs, act_dtype):
     """Scale of an attention output whose value sum is pv_abs = sum_j p_j |v_j|: the fp32 arithmetic, plus P rounded to the
     16-bit operand type for the P.V MMA (u_act * sum_j p_j |v_j|, expressed in units of 2^-24)."""
     return pv_abs * (1.0 + U[act_dtype] / EPS32)
 
 
-def check(y, ref, scale, kappa, name="", approx=None):
+def check(y, ref, scale, kappa, name="", approx=None, steps=None):
     """Asserts the per-element bound for kernel output `y` against the float64 reference `ref` (same shape); `approx` adds an
-    approximation error a kernel states for itself (a polynomial activation). Returns the worst ratio of error to bound over
-    the finite elements, and prints it (pytest -s lists it per op and build)."""
+    approximation error a kernel states for itself (a polynomial activation), `steps` tc_gemm's k-loop term (gemm_step_sums,
+    times GEMM_STEP). Returns the worst ratio of error to bound over the finite elements, and prints it (pytest -s lists it
+    per op and build)."""
     kappa = KAPPA[kappa] if isinstance(kappa, str) else kappa
     ref = ref.double().to(y.device)
     scale = scale.double().to(y.device).expand_as(ref)
     yd = y.double()
     e_acc = kappa * EPS32 * scale
+    if steps is not None:
+        e_acc = e_acc + GEMM_STEP * EPS32 * steps.double().to(y.device)
     if approx is not None:
         e_acc = e_acc + approx.double().to(y.device)
     bound = U[y.dtype] * ref.abs() + ETA[y.dtype] + e_acc
@@ -76,7 +105,8 @@ def check(y, ref, scale, kappa, name="", approx=None):
         i = bad.flatten().nonzero()[0].item()
         idx = tuple(int(v) for v in torch.unravel_index(torch.tensor(i), ref.shape))
         raise AssertionError(f"{name}: {int(bad.sum())} of {ref.numel()} elements outside |y - ref| <= u_out |ref| + "
-                             f"eta + {kappa:g} 2^-24 scale; first at {idx}: y {yd[idx].item():.9g}, ref {ref[idx].item():.9g}, "
+                             f"eta + {kappa:g} 2^-24 scale{' + k-step term' if steps is not None else ''}; first at {idx}: "
+                             f"y {yd[idx].item():.9g}, ref {ref[idx].item():.9g}, "
                              f"bound {bound[idx].item():.3g}, {int(must_inf.sum())} elements must overflow to inf; "
                              f"worst error/bound {ratio:.3g}")
     print(f"error/bound {name} [{y.dtype}]: {ratio:.3f}")
