@@ -56,7 +56,7 @@ _SIGS = {
     "gcd_clip_preprocess": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                     c_void_p, c_int, c_void_p]),
     "gcd_attention_temporal": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
-    "gcd_softmax_rows": (c_int, [c_void_p, c_int64, c_int, c_float, c_void_p, c_void_p]),
+    "gcd_softmax_rows": (c_int, [c_void_p, c_int64, c_int, c_float, c_float, c_void_p, c_void_p]),
     "gcd_memset_async": (c_int, [c_void_p, c_int, c_int64, c_void_p]),
     "gcd_cast_f32_to_act": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
     "gcd_upsample2x_to_act": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

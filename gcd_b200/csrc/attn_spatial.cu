@@ -81,6 +81,12 @@ attn_kernel(const __grid_constant__ CUtensorMap mapQKV, const Params p) {
     const int r0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);    // tile row of this thread's first accumulator row (+8: second)
     const int cb = 2 * (lane & 3);
     constexpr float SCALE_LOG2 = 0.125f * 1.4426950408889634f;
+    // P is packed to 16 bits as 2^15 exp(s - m), not exp(s - m): fp16 would flush weights below 2^-25 of the row maximum to 0 (and
+    // keep those below 2^-14 as subnormals), losing the mass of many keys 17+ nats below a dominant one. With the offset the
+    // largest weight is 32768 < 65504 and the flush threshold drops to 2^-40; l carries the same power of two, so O / l is
+    // unchanged. The running maximum m_run is kept shifted by -P_LOG2 (the shift rides on the block maximum's multiply), so the
+    // offset costs no instruction; alpha, a difference of two shifted maxima, is the same.
+    constexpr float P_LOG2 = 15.f;
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
     float o[32];
 #pragma unroll
@@ -117,13 +123,13 @@ attn_kernel(const __grid_constant__ CUtensorMap mapQKV, const Params p) {
             for (int i = 0; i < 8; i++) mx = fmaxf(mx, fmaxf(sv[4 * i + 2 * h], sv[4 * i + 2 * h + 1]));
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-            const float m_new = fmaxf(m_run[h], mx * SCALE_LOG2);
+            const float m_new = fmaxf(m_run[h], fmaf(mx, SCALE_LOG2, -P_LOG2));   // row maximum (log2 units) - P_LOG2
             const float alpha = ex2(m_run[h] - m_new);   // 0 on the first block (m_run = -inf)
             m_run[h] = m_new;
             float ls = 0.f;
 #pragma unroll
             for (int i = 0; i < 8; i++) {
-                const float e0 = ex2(fmaf(sv[4 * i + 2 * h], SCALE_LOG2, -m_new));
+                const float e0 = ex2(fmaf(sv[4 * i + 2 * h], SCALE_LOG2, -m_new));   // 2^15 exp(s - m)
                 const float e1 = ex2(fmaf(sv[4 * i + 2 * h + 1], SCALE_LOG2, -m_new));
                 ls += e0 + e1;
                 // accumulator columns 8i..8i+7 = A columns 8(i&1).. of K step i>>1; register 2(i&1) + h

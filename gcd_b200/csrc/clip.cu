@@ -221,10 +221,13 @@ attn_d80_kernel(const act_t* __restrict__ qkv, int L, int heads, float scale_log
         l0 *= al0; l1 *= al1;
 #pragma unroll
         for (int i = 0; i < 10; i++) { o[i][0] *= al0; o[i][1] *= al0; o[i][2] *= al1; o[i][3] *= al1; }
+        // P = 2^15 exp2(s - m) (largest 32768): the offset keeps weights down to 2^-40 of the row maximum out of fp16's
+        // flush-to-zero range when P is packed for P.V; l carries the same power of two
+        const float ms0 = m0 - 15.f, ms1 = m1 - 15.f;
 #pragma unroll
         for (int j = 0; j < 8; j++) {
-            s[j][0] = exp2f(s[j][0] - m0); s[j][1] = exp2f(s[j][1] - m0);
-            s[j][2] = exp2f(s[j][2] - m1); s[j][3] = exp2f(s[j][3] - m1);
+            s[j][0] = exp2f(s[j][0] - ms0); s[j][1] = exp2f(s[j][1] - ms0);
+            s[j][2] = exp2f(s[j][2] - ms1); s[j][3] = exp2f(s[j][3] - ms1);
             l0 += s[j][0] + s[j][1];
             l1 += s[j][2] + s[j][3];
         }

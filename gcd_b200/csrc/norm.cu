@@ -438,8 +438,9 @@ extern "C" int gcd_layernorm_f32(const float* in, int64_t rows, int C, const flo
 }
 
 // ---------------------------------------------------------------------------------------------- row softmax
-// model.py:161-201 AttnBlock: softmax(q k^T / sqrt(512)) with 9216 columns; one block per row, fp32 in, act out.
-__global__ void softmax_rows_kernel(const float* __restrict__ in, int cols, float scale, act_t* __restrict__ out) {
+// model.py:161-201 AttnBlock: softmax(q k^T / sqrt(512)) with 9216 columns; one block per row, fp32 in, act out (times
+// out_scale: the VAE stores 2^15 P, so that fp16 keeps weights down to 2^-40 out of its flush-to-zero range).
+__global__ void softmax_rows_kernel(const float* __restrict__ in, int cols, float scale, float out_scale, act_t* __restrict__ out) {
     __shared__ float red[32];
     const int64_t row = blockIdx.x;
     const float* src = in + row * (int64_t)cols;
@@ -460,13 +461,13 @@ __global__ void softmax_rows_kernel(const float* __restrict__ in, int cols, floa
     __syncthreads();
     s = 0.f;
     for (int i = 0; i < (blockDim.x >> 5); i++) s += red[i];
-    const float inv = 1.0f / s;
+    const float inv = out_scale / s;
     act_t* dst = out + row * (int64_t)cols;
     for (int j = threadIdx.x; j < cols; j += blockDim.x) dst[j] = f2act(__expf((src[j] - m) * scale) * inv);
 }
-extern "C" int gcd_softmax_rows(const float* in, int64_t rows, int cols, float scale, void* out, void* stream) {
+extern "C" int gcd_softmax_rows(const float* in, int64_t rows, int cols, float scale, float out_scale, void* out, void* stream) {
     GCD_REQUIRE(rows < (1ll << 31), "softmax_rows: too many rows");
-    softmax_rows_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(in, cols, scale, (act_t*)out);
+    softmax_rows_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(in, cols, scale, out_scale, (act_t*)out);
     GCD_CUDA_CHECK(cudaGetLastError());
     g_launches++;
     return 0;

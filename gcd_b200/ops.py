@@ -250,12 +250,13 @@ def layernorm_f32(x, gamma, beta, out, eps=1e-5, add=None, add_rows_per=1, add_m
                                       int(add_mod), _p(out), _stream()), "layernorm_f32")
 
 
-def softmax_rows(x, scale, out):
+def softmax_rows(x, scale, out, out_scale=1.0):
+    """out = out_scale * softmax(x * scale) per row: x float32 [rows, cols], out act."""
     _need_cuda(x, out)
     rows, cols = x.shape
     assert x.dtype == torch.float32 and x.is_contiguous() and out.is_contiguous()
     with _timed("elem", 0.0, rows * cols * 10):
-        check(lib().gcd_softmax_rows(_p(x), rows, cols, float(scale), _p(out), _stream()), "softmax_rows")
+        check(lib().gcd_softmax_rows(_p(x), rows, cols, float(scale), float(out_scale), _p(out), _stream()), "softmax_rows")
 
 
 # ------------------------------------------------------------------------------------------------ attention

@@ -17,6 +17,12 @@ from . import ops, spec
 from .engine import Engine, EngineCache, need_option, reference_base, register_param_tree
 
 
+# The mid attention stores its probabilities as P_SCALE * P: fp16 flushes weights below 2^-25 to zero, P_SCALE * P only below
+# 2^-40 (the largest stored value is 32768 < 65504). The P.V GEMM takes the factor back out in its epilogue (a_acc, applied after
+# the bias, with the bias packed as P_SCALE * b_v); powers of two, so nothing else rounds differently.
+P_SCALE = 2.0 ** 15
+
+
 class _VAEEngine(Engine):
     """What the VAE encoder and decoder share: channels-last fp32 residual stream, 16-bit tensor-core operands, the spatial
     ResnetBlock and the mid AttnBlock."""
@@ -37,6 +43,7 @@ class _VAEEngine(Engine):
         self._norm(sd, p + ".norm", p + ".norm")
         for n in ("q", "k", "v", "proj_out"):
             self._lin(sd, f"{p}.{n}", f"{p}.{n}")
+        self.w[p + ".v.b_p"] = self.w[p + ".v.b"] * P_SCALE
 
     def _res2d(self, p, x, cin, cout, n, H, Wd, tag, out_geom, x_stats=None):
         """ResnetBlock.forward with temb=None (model.py:127-151). `out_geom`: (images, rows per image) of the GroupNorm that
@@ -83,9 +90,10 @@ class _VAEEngine(Engine):
             sc = pool.get("attn_s", (fc * S, S), torch.float32)[: (f1 - f0) * S]
             pr = pool.get("attn_p", (fc * S, S), AD)[: (f1 - f0) * S]
             ops.bmm_nt(q[f0 * S:f1 * S].view(f1 - f0, S, C), k[f0 * S:f1 * S].view(f1 - f0, S, C), ops.make_ep(sc))
-            ops.softmax_rows(sc, C ** -0.5, pr)
+            ops.softmax_rows(sc, C ** -0.5, pr, out_scale=P_SCALE)
             # softmax rows sum to 1 => the v bias contributes exactly +b_v to every output row
-            ops.bmm_nt(pr.view(f1 - f0, S, S), vt[f0:f1], ops.make_ep(o[f0 * S:f1 * S], bias=W[p + ".v.b"]))
+            ops.bmm_nt(pr.view(f1 - f0, S, S), vt[f0:f1],
+                       ops.make_ep(o[f0 * S:f1 * S], bias=W[p + ".v.b_p"], a_acc=1.0 / P_SCALE))
         ops.linear(o, W[p + ".proj_out.w"], ops.make_ep(x, bias=W[p + ".proj_out.b"], res1=x))
         return x
 

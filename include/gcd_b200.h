@@ -122,8 +122,10 @@ int gcd_attention_temporal(const void* qkv, int clips, int T, int tokens, int he
  * qkv: act [n, L, 3*heads*80] = in_proj output (q | k | v, head index outer within each third); out: act [n, L, heads*80].
  * L in 1..1024. */
 int gcd_attention_d80(const void* qkv, int n, int L, int heads, void* out, void* stream);
-/* Row softmax of float32 scores [rows, cols] * scale -> act probs (model.py:161-201 AttnBlock, d=512 single head). */
-int gcd_softmax_rows(const float* in, int64_t rows, int cols, float scale, void* out, void* stream);
+/* Row softmax of float32 scores [rows, cols] * scale -> act out_scale * probs (model.py:161-201 AttnBlock, d=512 single head).
+ * out_scale = 1 gives the probabilities. The VAE passes 2^15 (and undoes it in the P.V GEMM's epilogue, a_acc = 2^-15): fp16
+ * flushes probabilities below 2^-25 to zero, 2^15 P only below 2^-40; the largest stored value is then 32768 < 65504. */
+int gcd_softmax_rows(const float* in, int64_t rows, int cols, float scale, float out_scale, void* out, void* stream);
 
 /* ---- element-wise / layout ------------------------------------------------------------------------------- */
 int gcd_memset_async(void* p, int value, int64_t bytes, void* stream);

@@ -22,6 +22,14 @@ the running sum grows evenly (1.5e-4 of the result at K = 23040). The bound of a
 GEMM_STEP = 8 allows four truncations of under one fp32 ulp (2^-23 |P_i|) per k16 step, about twice the measured worst case.
 Tests that leave `steps` out hold the kernel to kappa alone; they use zero-mean operands.
 
+Attention packs its softmax weights P to the 16-bit operand type for the P.V MMA. Besides the relative rounding (u_act), a packed
+weight below fp16's normal range keeps only an absolute accuracy: half the subnormal spacing of the packed value. The kernels pack
+2^15 P, so that weight is ETA_P = 2^-25 / 2^15 = 2^-40 in units of the largest weight of the row (the flash kernels, whose P is
+relative to the row maximum) or of 1 (softmax_rows, whose P is normalised). The output moves by at most ETA_P * c * sum_j |v_j|
+with c = p_max or 1 (attention_scale). Packed without the offset, keys 17.3+ nats below a dominant one were flushed to zero, and
+a row whose dominant key has |v| ~ 0 and whose other keys carry |v| of 1-4 lost most of its output: up to 110 times the bound
+at 9216 keys, measured on one H100 80GB HBM3 (tests/test_attention_edges_gpu.py).
+
 A 16-bit fp16 output whose reference rounds past the fp16 maximum must be exactly the infinity of the reference's sign
 (IEEE round-to-nearest); within the accumulation error of the overflow threshold either outcome is accepted. bf16 has
 fp32's exponent range, so every bf16 output of these tests must be finite.
@@ -31,12 +39,15 @@ import torch
 U = {torch.float16: 2.0 ** -11, torch.bfloat16: 2.0 ** -8, torch.float32: 0.0}
 ETA = {torch.float16: 2.0 ** -25, torch.bfloat16: 2.0 ** -134, torch.float32: 0.0}
 EPS32 = 2.0 ** -24                    # fp32 unit roundoff
+P_OFFSET = 2.0 ** 15                  # attention packs 2^15 P to 16 bits (largest weight 32768)
+ETA_P = {t: e / P_OFFSET for t, e in ETA.items()}   # half the subnormal spacing of packed P, in units of P (2^-40 in fp16)
 FP16_OVERFLOW = 65520.0               # the smallest magnitude that rounds to inf in fp16 (65504 + half an ulp)
 
 # kappa per op class, in units of 2^-24 * scale (attention: the scale carries P's 16-bit repack, see attention_scale)
 KAPPA = {
     "gemm": 32.0,          # tc_gemm: Linear / conv / bmm with the fused epilogue (fp32 accumulation in the tensor cores)
-    "attention": 16.0,     # spatial / temporal / d80 flash attention (near one-hot rows with fp16-subnormal outputs reach ~10)
+    "attention": 16.0,     # spatial / temporal / d80 flash attention, softmax_rows + P.V (near one-hot rows with
+                           # fp16-subnormal outputs reach ~10); the scale carries P's 16-bit pack, subnormal range included
     "norm": 32.0,          # GroupNorm (fp64 sums from each element on) / LayerNorm (two-pass fp32), fp32 normalisation
     "elementwise": 8.0,    # softmax rows, CLIP preprocessing
 }
@@ -69,10 +80,14 @@ def gemm_step_sums(a, w, step=16):
     return total
 
 
-def attention_scale(pv_abs, act_dtype):
+def attention_scale(pv_abs, act_dtype, v_abs=None, c=1.0):
     """Scale of an attention output whose value sum is pv_abs = sum_j p_j |v_j|: the fp32 arithmetic, plus P rounded to the
-    16-bit operand type for the P.V MMA (u_act * sum_j p_j |v_j|, expressed in units of 2^-24)."""
-    return pv_abs * (1.0 + U[act_dtype] / EPS32)
+    16-bit operand type for the P.V MMA (u_act * sum_j p_j |v_j|), plus, when v_abs = sum_j |v_j| is given, packed weights in
+    the subnormal range (ETA_P * c * sum_j |v_j|, c = p_max for the flash kernels, 1 for softmax_rows); in units of 2^-24."""
+    s = pv_abs * (1.0 + U[act_dtype] / EPS32)
+    if v_abs is not None:
+        s = s + (ETA_P[act_dtype] / EPS32) * c * v_abs
+    return s
 
 
 def check(y, ref, scale, kappa, name="", approx=None, steps=None):

@@ -3,7 +3,7 @@
 The module fixture builds it next to the default library as gcd_b200/libgcd_b200_bf16.so (objects under gcd_b200/build/bf16/;
 an up-to-date library is reused) and the tests run child Pythons that load it through GCD_LIB_PATH: one GEMM and the dtype
 guards directly, then the kernel parity suites (test_ops_gpu.py, test_tc_pingpong_gpu.py, test_tc_accumulation_gpu.py,
-test_lpips_gpu.py and the op tests of test_clip_gpu.py), whose per-element bounds follow the operand type
+test_attention_edges_gpu.py, test_lpips_gpu.py and the op tests of test_clip_gpu.py), whose per-element bounds follow the operand type
 (oracle/error_model.py).
 
 The model-level goldens (UNet, VAE, CLIP tower, sampler trajectories) are not run on the bf16 build: their bars are fitted to
@@ -71,7 +71,7 @@ def test_bf16_library_loads_and_computes(bf16_env):
 
 def test_bf16_kernel_parity_suite(bf16_env):
     targets = ["tests/test_ops_gpu.py", "tests/test_tc_pingpong_gpu.py", "tests/test_tc_accumulation_gpu.py",
-               "tests/test_lpips_gpu.py"]
+               "tests/test_attention_edges_gpu.py", "tests/test_lpips_gpu.py"]
     targets += [f"tests/test_clip_gpu.py::{t}" for t in CLIP_OP_TESTS]
     r = subprocess.run(_python() + ["-m", "pytest", "-q", "-s", "-p", "no:cacheprovider"] + targets, cwd=ROOT, env=bf16_env,
                        capture_output=True, text=True, timeout=3000)
